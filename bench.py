@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — premises encoded/s (reindex) and retrieve() queries/s on B200s, next to the
+"""bench.py — premises encoded/s (reindex) and retrieve() queries/s on H100s, next to the
 reference's own CPU path.
 
     python bench.py --gpus 1 --steps K --warmup W            # engine arm
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # ... and write what the last timed step computed
     python bench.py --impl reference --steps K --warmup W    # reference arm (HF CPU path)
     torchrun --nproc-per-node N ... bench.py --gpus N ...    # one rank per GPU
 
@@ -19,7 +20,8 @@ weights (seed 3407).  Every step uses a fresh slice of the corpus; the per-step 
          of Premise objects, then `.cpu()` of the index as retrieval/index.py:37 does): host
          strings -> pinned bytes -> H2D -> engine -> D2H inside the timed region.
   retrieve   extra leg, BASELINE configs[2]/[3]: 1024 states x 200k-premise (per GPU) bf16 index,
-         k = 100, fused sim+top-k (+ all-gather + merge when N > 1): queries/s and roofline, plus a
+         k = 100, fused sim+top-k (+ all-gather + merge when N > 1), timed over K calls after
+         max(10, W) warm-up calls: queries/s and roofline, plus a
          `parity` object: 64 sampled queries re-ranked by brute force (fp64 Q.E^T of every rank's shard,
          all-gathered, exact top-k) against the engine's merged result on EVERY rank — a mismatch makes
          the run exit non-zero.
@@ -29,6 +31,12 @@ weights (seed 3407).  Every step uses a fresh slice of the corpus; the per-step 
          200k-premise corpus: encode of one state + access bitmask + top-k + Premise objects.
   sweep (N = 1)  BASELINE configs[4]: encoder throughput at seq_len {128,512,1024,2048} x batch {32,128,512}.
   reindex_2048 (N = 1)  the shape retrieval/index.py:33 indexes at: max_seq_len 2048, token length ~ U[17, 2048].
+
+`--dump-outputs DIR` writes, after the timed steps, what a caller of the timed paths receives from the last
+step, as float32 / float64 .npy files (rank 0): `embeddings.npy` (the re-indexed premises of the last device
+step, float32; a fixed seeded sample of rows, listed in `embedding_rows.npy`, when the step's embeddings
+exceed 48 MB) and, with the retrieve leg, `retrieve_scores.npy` (fp64) / `retrieve_indices.npy` of the last
+1024-state call.  Inputs are seeded, so two builds run with the same arguments can be compared file by file.
 """
 from __future__ import annotations
 
@@ -69,12 +77,18 @@ def encoder_flops(token_lens: np.ndarray) -> float:
 
 
 def load_peaks():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        d = json.loads(p.read_text())
-        return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"],
-                "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback"}
+    """NVIDIA's H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16.  No sustained rate
+    is published; a power-limited card holds less than the data-sheet rate, so fractions of it are lower bounds."""
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "H100 SXM data sheet"}
+
+
+EMB_DUMP_BYTES = 48 << 20   # the rest of the 64 MB dump budget holds the retrieve results
+
+
+def dump_outputs(out_dir: Path, arrays: dict) -> None:
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 class ClockSampler:
@@ -122,6 +136,16 @@ class ClockSampler:
         # samples taken while the GPU was busy are the upper half of the clock distribution
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "samples": len(sm), "reasons": sorted(reasons)}
+
+
+def gpu_info(index: int) -> dict:
+    """Board name and power limit: a time or rate measured here is only meaningful next to them."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1])}
+    except (OSError, subprocess.SubprocessError, ValueError, IndexError):
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
 
 
 def dist_env():
@@ -219,11 +243,16 @@ def run_engine(args) -> dict:
     ffn = prof["ffn_up_gemm"]
     ffn_flops = 2.0 * timed_tokens * 7168 * 1472 * cfg["num_layers"]
     ffn_tf = ffn_flops / (ffn["ms"] / 1e3) / 1e12 if ffn["ms"] > 0 else 0.0
-    traffic = None
-    tpath = ROOT / "profiles" / "roofline_traffic.json"
-    if tpath.exists():
-        traffic = json.loads(tpath.read_text()).get("ffn_up_gemm_dram_bytes_per_launch")
     launches = sum(v["launches"] for v in prof.values())
+
+    dumps = {}
+    if args.dump_outputs and rank == 0:
+        emb = out.float().cpu().numpy()                       # the last timed step's premises, in corpus order
+        if emb.nbytes > EMB_DUMP_BYTES:
+            rows = np.sort(np.random.default_rng(synth.SEED).choice(P, EMB_DUMP_BYTES // (D_MODEL * 4), replace=False))
+            emb = emb[rows]
+            dumps["embedding_rows"] = rows.astype(np.float64)
+        dumps["embeddings"] = emb
 
     # ---- end to end through the public API (host strings in, host index out)
     e2e = None
@@ -277,7 +306,8 @@ def run_engine(args) -> dict:
         E = synth.random_unit_rows(n_idx, D_MODEL, 1000 + rank, dev)
         handle = IndexHandle(E)
         Q_all = synth.random_unit_rows(1024, D_MODEL, 999, dev)   # same queries on every rank
-        retrieve = retrieve_leg(Q_all, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_parity=True)
+        retrieve = retrieve_leg(Q_all, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_parity=True,
+                                dumps=dumps if args.dump_outputs and rank == 0 else None)
         retrieve_q64 = retrieve_leg(Q_all[:64].contiguous(), E, handle, k, rank, world, dev, peaks, e0, e1, K, W)
         retrieve_q1 = retrieve_leg(Q_all[:1].contiguous(), E, handle, k, rank, world, dev, peaks, e0, e1, K, W)
         retrieve["guard"] = handle.stats()
@@ -306,12 +336,12 @@ def run_engine(args) -> dict:
                              "frac": timed_flops / (ms_dev / 1e3) / 1e12 / peaks["tf_sustained"],
                              "note": "WHOLE PATH: algorithmic FLOPs sum F(l_i) of SURVEY 8d over the whole step (per GPU) / step time; "
                                      "`roofline` below is the dominant kernel alone"},
-        "roofline": {"bound": "tensor", "kernel": "gemm_tc2_kernel<6,EpiGeGLU> (FFN up-projection, 2-CTA tcgen05, 58% of FLOPs)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_tc_kernel<128,4,EpiGeGLUT<64>,split-B> (FFN up-projection, wgmma, 58% of FLOPs)",
                      "achieved": ffn_tf, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
-                     "frac": ffn_tf / peaks["tf_sustained"], "peak_source": peaks["source"] + " (sustained bf16)",
-                     "traffic": traffic, "launches": ffn["launches"], "avg_launch_ms": ffn["ms"] / max(ffn["launches"], 1)},
+                     "frac": ffn_tf / peaks["tf_sustained"], "peak_source": peaks["source"] + " (dense bf16)",
+                     "launches": ffn["launches"], "avg_launch_ms": ffn["ms"] / max(ffn["launches"], 1)},
         "kernel_ms": {k2: v["ms"] for k2, v in prof.items()},
-        "e2e": e2e, "gpu_launches": launches, "clocks": clocks, "retrieve": retrieve,
+        "e2e": e2e, "gpu_launches": launches, "gpu": gpu_info(local), "clocks": clocks, "retrieve": retrieve,
         "retrieve_q1": retrieve_q1, "retrieve_q64": retrieve_q64, "retrieve_single": retrieve_single,
         "sweep": sweep, "reindex_2048": reindex_2048,
     }
@@ -320,6 +350,9 @@ def run_engine(args) -> dict:
         exc = SystemExit(f"[bench] retrieve parity FAILED: {parity}")
         exc.bench_result = result if rank == 0 else None
         raise exc
+    if dumps:
+        dump_outputs(Path(args.dump_outputs), dumps)
+        result["dump_outputs"] = {name: list(a.shape) for name, a in dumps.items()}
     if rank == 0 and world == 1 and not args.skip_cpu_baseline:
         result["cpu_baseline"] = cpu_baseline_encode(cfg, sd, data, offsets, n_premises=args.cpu_sample)
     if world > 1:
@@ -366,15 +399,15 @@ def brute_force_parity(Q, E, k, rank, world, dev, got_idx, got_s64, n_sample=64)
     return out
 
 
-def retrieve_leg(Q, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_parity=False):
+def retrieve_leg(Q, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_parity=False, dumps=None):
     from reprover_b200.dist import sharded_topk
     from reprover_b200.retrieval_ops import sim_topk
 
     nq, n_idx = Q.shape[0], E.shape[0]
     Q_host = Q.cpu().pin_memory()
-    # one retrieve is 0.1-0.6 ms: a handful of repetitions would be timed while the SM clock is still
-    # ramping after the host-side legs; 50 repetitions after 10 warm-ups are past that
-    reps, warm_r = max(50, K), max(10, W)
+    # one retrieve is well under a millisecond: at least 10 warm-up calls let the SM clock ramp up after the
+    # host-side legs before the K timed calls
+    reps, warm_r = K, max(10, W)
 
     def retrieve_dev(q=Q):
         if world == 1:
@@ -387,10 +420,13 @@ def retrieve_leg(Q, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_p
     barrier(world)
     e0.record()
     for _ in range(reps):
-        retrieve_dev()
+        last = retrieve_dev()
     e1.record()
     barrier(world)
     ms_r = max_over_ranks(e0.elapsed_time(e1), world, dev) / reps
+    if dumps is not None:
+        dumps["retrieve_scores"] = last[3].cpu().numpy().astype(np.float64)
+        dumps["retrieve_indices"] = last[1].cpu().numpy().astype(np.float64)
     # e2e: queries from pinned host memory, results back to the host
     res_scores = torch.empty(nq, k, dtype=torch.float32).pin_memory()
     res_idx = torch.empty(nq, k, dtype=torch.int64).pin_memory()
@@ -418,7 +454,7 @@ def retrieve_leg(Q, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_p
     leg = {
         "metric": "retrieve queries/s", "config": {"queries": nq, "index_rows_per_gpu": n_idx, "index_rows_total": n_idx * world,
                                                   "k": k, "dtype": "bf16", "merge": "nccl all_gather + device merge" if world > 1 else "none",
-                                                  "path": "streaming kernel (HBM-bound)" if nq <= 2 else "tcgen05 MMA + fused top-k",
+                                                  "path": "streaming kernel (HBM-bound)" if nq <= 2 else "wgmma + fused top-k",
                                                   "warmup": warm_r, "repetitions": reps, "l2": "index (589 MB) larger than L2"},
         "value": nq / (ms_r / 1e3), "ms": ms_r,
         "e2e": {"value": nq / (ms_re / 1e3), "ms": ms_re, "h2d_bytes": nq * D_MODEL * 2, "d2h_bytes": nq * k * 12},
@@ -427,16 +463,10 @@ def retrieve_leg(Q, E, handle, k, rank, world, dev, peaks, e0, e1, K, W, check_p
                      "peak": peaks["tf_burst"] if bound == "tensor" else peaks["hbm_gbs"],
                      "unit": "TFLOP/s" if bound == "tensor" else "GB/s",
                      "frac": max(t_mma, t_hbm) / (ms_r / 1e3), "hbm_frac": t_hbm / (ms_r / 1e3),
-                     # the same against the sustained tensor rate (what a power-capped B200 holds over a step)
                      "frac_of_sustained": (max(flops / (peaks["tf_sustained"] * 1e12), t_hbm) / (ms_r / 1e3)) if bound == "tensor" else None,
                      "algorithmic_bytes": bytes_alg, "peak_source": peaks["source"] + (" (burst bf16)" if bound == "tensor" else ""),
                      "note": "whole retrieve (every launch of the call [+ all-gather + merge]) vs max(t_MMA, t_HBM) of one pass over the index"},
     }
-    if bound == "hbm" and nq <= 2:
-        tpath = ROOT / "profiles" / "roofline_traffic.json"
-        if tpath.exists():
-            leg["roofline"]["traffic"] = json.loads(tpath.read_text()).get("smallq_topk_dram_bytes_per_launch")
-            leg["roofline"]["kernel"] = "smallq_topk_kernel<1,6> (one streaming pass over the bf16 index, fused per-warp heaps + fp64 re-score + rank)"
     if check_parity:
         r = retrieve_dev()
         torch.cuda.synchronize()
@@ -521,7 +551,7 @@ def sweep_leg(eng, dev, peaks):
             rows.append({"seq_len": L, "batch": B, "ms": ms, "seq_per_s": B / ms * 1e3, "tflops": tf,
                          "frac_of_sustained_peak": tf / peaks["tf_sustained"], "reps": reps})
     return {"metric": "encoder sequences/s and roofline fraction, BASELINE configs[4]", "peak": peaks["tf_sustained"],
-            "peak_source": peaks["source"] + " (sustained bf16)", "rows": rows,
+            "peak_source": peaks["source"] + " (dense bf16)", "rows": rows,
             "frac_min": min(r["frac_of_sustained_peak"] for r in rows), "frac_max": max(r["frac_of_sustained_peak"] for r in rows)}
 
 
@@ -654,6 +684,8 @@ def main():
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--skip-extras", action="store_true", help="skip retrieve_single / sweep / reindex_2048 (N = 1 legs)")
     ap.add_argument("--tmp", default="/tmp/rpx_bench")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs as .npy files into DIR")
     args = ap.parse_args()
     if args.impl == "engine" and args.warmup < 3:
         print(f"[bench] --warmup {args.warmup} raised to 3 (timing rules: at least 3 warm-up steps)", file=sys.stderr)

@@ -1,4 +1,4 @@
-/* rpx.h — C ABI of the B200-native premise-retrieval engine (librpx.so).
+/* rpx.h — C ABI of the H100-native premise-retrieval engine (librpx.so).
  *
  * The reference (lean-dojo/ReProver) has NO plugin / operator / FFI interface for
  * this path: its seam is the Python attribute surface of `PremiseRetriever`
@@ -19,7 +19,7 @@
  *   - `stream` is a cudaStream_t passed as void*.  All work is enqueued on it;
  *     functions return without synchronising unless stated.
  *   - Handles are not thread-safe per handle; distinct handles are independent.
- *   - sm_100a (B200) only.  There is no CPU or other-GPU fallback: calling a
+ *   - sm_90a (H100) only.  There is no CPU or other-GPU fallback: calling a
  *     compute entry point without such a device fails with RPX_ERR_CUDA /
  *     RPX_ERR_UNSUPPORTED.
  */
@@ -49,7 +49,7 @@ enum { RPX_DTYPE_BF16 = 0, RPX_DTYPE_F32 = 1 };
 /* Last error message of the calling thread ("" if none). */
 const char* rpx_last_error(void);
 int rpx_version(void);
-/* RPX_OK iff the current CUDA device is compute capability 10.x. */
+/* RPX_OK iff the current CUDA device is compute capability 9.0. */
 int rpx_device_check(void);
 
 /* ------------------------------------------------------------------------- encoder
@@ -132,10 +132,10 @@ int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* 
 
 /* Latency path: encode calls with at most `max_tokens` packed tokens (0 = never, the default) run on
  * kernels shaped for ONE proof state — the reference's per-state call (`retrieve`,
- * retrieval/model.py:348-357) — instead of the 256 x 256 pair tiles that are sized for re-indexing: narrow
- * 1-CTA GEMM tiles (64 or 128 tokens x 64 columns, 128 x 128 for the gated FFN-up) that spread the state's work
- * over 70-140 SMs, attention on 32-query CTAs whose four softmax warps share the key range, pooling as
- * per-group partial rows, everything chained by programmatic dependent launch.  Results agree with the
+ * retrieval/model.py:348-357) — instead of the 128 x 128 tiles that are sized for re-indexing: narrow
+ * GEMM tiles (64 or 128 tokens x 64 columns, 128 x 128 for the gated FFN-up) that spread the state's work
+ * over most of the SMs, the next layer's weights prefetched into L2 by the idle SMs, pooling as per-group
+ * partial rows, everything chained by programmatic dependent launch.  Results agree with the
  * throughput path to a few 1e-4 on unit-norm embeddings (the RMSNorm statistics are summed in another
  * grouping, which flips the odd bf16 rounding of an intermediate), not bit for bit, so a caller that needs
  * re-indexing's bits leaves it off; within the latency path a sequence's embedding does not depend on what
@@ -193,7 +193,7 @@ int rpx_index_destroy(rpx_index* ix);
 int rpx_index_stats(rpx_index* ix, void* stream, float* h_norm_max, float* h_max_err, float* h_max_eps,
                     int64_t* h_n_exact);
 
-/* Path selection flags of rpx_index_topk (0 = automatic: streaming kernel for nq <= 2, tcgen05
+/* Path selection flags of rpx_index_topk (0 = automatic: streaming kernel for nq <= 2, tensor-core
  * kernel otherwise, exact pass for k > 200).  The forcing flags exist for parity tests. */
 enum { RPX_TOPK_AUTO = 0, RPX_TOPK_FORCE_MMA = 1, RPX_TOPK_FORCE_STREAM = 2, RPX_TOPK_FORCE_EXACT = 4 };
 
@@ -242,11 +242,12 @@ int rpx_topk_merge_packed(const int64_t* d_packed, int32_t n_parts, int32_t nq, 
 int rpx_debug_set_timeline(unsigned long long* d_stamps, int32_t n_slots);
 
 /*
- * Plain tcgen05 GEMM used by the parity tests of the contraction core:
+ * Plain wgmma GEMM used by the parity tests of the contraction core:
  * C[M, N] (fp32, ldc = N) = A[M, K] * B[N, K]^T, bf16 inputs; K % 64 == 0, N % 32 == 0. */
 int rpx_gemm_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                       int32_t K, void* stream);
-/* Same contract through the 2-CTA (cta_group::2, 256 x 256 tile) form of the core. */
+/* Same contract through the paired form of the core: clusters of two CTAs on vertically adjacent
+ * 128 x 128 tiles that share each B tile through TMA multicast. */
 int rpx_gemm2_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                        int32_t K, void* stream);
 

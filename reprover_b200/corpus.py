@@ -112,7 +112,7 @@ class Premise:
 
         Like the reference, the name is used as a regex pattern UN-escaped (its dots match any
         character).  Compiling one or two fresh patterns per premise costs ~90 us, which would cap
-        re-indexing at ~11 k premises/s per host thread — below what one B200 encodes — so names
+        re-indexing at ~11 k premises/s per host thread — below what one GPU encodes — so names
         made of ordinary components (no regex metacharacter, quote or space: all but a handful of
         Lean names) take `_sub_plain`, a direct scan with exactly `re.sub`'s semantics for that
         pattern shape (pinned against `re.sub` in tests/test_host_cpu.py)."""

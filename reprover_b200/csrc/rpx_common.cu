@@ -200,8 +200,8 @@ int get_device_info(DeviceInfo* out) {
     cache[dev] = d;
   }
   *out = cache[dev];
-  RPX_REQUIRE(out->cc_major == 10, RPX_ERR_UNSUPPORTED,
-              "device %d is sm_%d%d; this engine is sm_100a (B200) only", dev, out->cc_major,
+  RPX_REQUIRE(out->cc_major == 9 && out->cc_minor == 0, RPX_ERR_UNSUPPORTED,
+              "device %d is sm_%d%d; this engine is sm_90a (H100) only", dev, out->cc_major,
               out->cc_minor);
   return RPX_OK;
 }

@@ -65,7 +65,7 @@ struct DeviceInfo {
   int cc_major = 0, cc_minor = 0;
   size_t smem_optin = 0;
 };
-// Properties of the current device (cached per device ordinal).  Fails unless sm_100.
+// Properties of the current device (cached per device ordinal).  Fails unless sm_90.
 int get_device_info(DeviceInfo* out);
 
 // Debug timeline (rpx_debug_set_timeline): each 1-CTA GEMM launch gets the next 8-stamp slot of the buffer.
@@ -73,7 +73,7 @@ unsigned long long* next_timeline_slot();
 
 // Programmatic dependent launch is used along the kernel chain of encode calls of up to 16 k tokens (the
 // kernels are short and their prologues are worth overlapping); full re-indexing chunks are launched
-// plainly (measured: neutral to -1 % there).  RPX_PDL=0 never, RPX_PDL=2 every encoder launch.
+// plainly (their kernels are long enough that the overlap does not pay).  RPX_PDL=0 never, RPX_PDL=2 every encoder launch.
 bool pdl_enabled();
 void set_pdl_scope(bool on);  // per thread: true while such a forward enqueues its kernels
 

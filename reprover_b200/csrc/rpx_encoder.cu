@@ -11,7 +11,7 @@
 //     h16  [T, D] bf16   same values, GEMM A operand
 //     qkv  [T, 3*H*64] bf16,  attn [T, H*64] bf16,  ffn [T, d_ff] bf16
 //     ssA / ssB [n_parts][T] fp32  per-row partial sums of h32^2, one per n-tile of the GEMM that
-//                             produced h32 (6 for d_model = 1472) -> RMSNorm row scale
+//                             produced h32 (12 for d_model = 1472) -> RMSNorm row scale
 // RMSNorm never runs as its own kernel: its weight vector is folded into the next
 // GEMM's B operand when the weights are packed, and the row scale rsqrt(mean(h^2)+eps)
 // is applied to the fp32 accumulator in that GEMM's epilogue (rpx_gemm.cuh RowScale).
@@ -27,83 +27,15 @@ namespace rpx {
 
 namespace {
 
-constexpr int kBlockN = 256;
-
-#ifndef RPX_GEMM_2CTA
-#define RPX_GEMM_2CTA 1
-#endif
-// The encoder's GEMMs: 2-CTA (cta_group::2) tiles by default, the 1-CTA kernel with -DRPX_GEMM_2CTA=0.
-template <class Epi>
-int encoder_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
-                 const typename Epi::Params& ep, cudaStream_t st) {
-#if RPX_GEMM_2CTA
-  return launch_gemm2<Epi>(A, lda, B, ldb, M, N, K, ep, st);
-#else
-  return launch_gemm<kBlockN, Epi>(A, lda, B, ldb, M, N, K, ep, st);
-#endif
-}
-
-// Residual-update GEMMs (attention output projection, FFN down projection).  With the 2-CTA kernel
-// the residual stream moves through TMA (EpiResidualTma: RPX_RES_RING boxes per warp, which leaves
-// room for RPX_RES_STAGES operand stages); -DRPX_RES_TMA=0 or a model too narrow for the ring's
-// look-ahead uses the register epilogue.
-#ifndef RPX_RES_TMA
-#define RPX_RES_TMA (RPX_GEMM_2CTA && RPX_EPI_WARPS == 4)
-#endif
-// The TMA epilogue pays for its ring with operand stages (4 instead of 6), which costs a
-// tensor-bound GEMM more than the epilogue gains: it is used while the MMA time of a tile
-// (~0.43 us per 64 of K) is below the ~7 us the tile's 320 KB of residual traffic need, i.e. for
-// the attention output projection (K = 384: 57.6 -> 38.5 ms per 4096-premise step) but not for the
-// FFN down projection (K = 3584: 99.8 ms with the register epilogue, 114 ms with this one).
-#ifndef RPX_RES_TMA_MAX_K
-#define RPX_RES_TMA_MAX_K 1024
-#endif
-#ifndef RPX_RES_RING
-#define RPX_RES_RING 4
-#endif
-#ifndef RPX_RES_STAGES
-#define RPX_RES_STAGES 4
-#endif
-using EpiResTma = EpiResidualTma<RPX_RES_RING>;
-
-struct ResidualMaps {
-  bool use_tma = false;
-  CUtensorMap h32, h16;
-};
-
-// Narrowest n-tile of the 2-CTA kernel for an N-column output (see n_tile_range).
-inline int min_tile_cols(int N) {
-  const int tiles_n = ceil_div(N, kBlockN);
-  return 32 * (ceil_div(N, 32) / tiles_n);
-}
-
-int make_residual_maps(ResidualMaps* m, float* h32, __nv_bfloat16* h16, int T, int D) {
-  m->use_tma = false;
-#if RPX_RES_TMA
-  if (D % 32 == 0 && min_tile_cols(D) >= 32 * (RPX_RES_RING - 1)) {
-    RPX_TRY(make_tmap_2d(&m->h32, 4, h32, (uint64_t)T, (uint64_t)D, (uint64_t)D, 32, 32, 128));
-    RPX_TRY(make_tmap_2d(&m->h16, 2, h16, (uint64_t)T, (uint64_t)D, (uint64_t)D, 32, 32, 64));
-    m->use_tma = true;
-  }
-#endif
-  return RPX_OK;
-}
+// Throughput-path tiles: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand ring fit the 227 KB of
+// shared memory an H100 block may use; the gated FFN up-projection runs them as split-B tiles of 64 hidden units.
+constexpr int kBlockN = 128;
 
 // h32 += A @ B^T, h16 = bf16(h32), ss = partial sums of h32^2 per n-tile.
-int residual_gemm(const ResidualMaps& maps, const void* A, int64_t lda, const void* B, int64_t ldb, int T, int D,
-                  int K, float* h32, __nv_bfloat16* h16, float* ss, cudaStream_t st) {
-#if RPX_RES_TMA
-  if (maps.use_tma && K <= RPX_RES_TMA_MAX_K) {
-    EpiResTma::Params ep;
-    ep.tm_h32 = maps.h32;
-    ep.tm_h16 = maps.h16;
-    ep.ss_out = ss;
-    ep.ss_stride = T;
-    return launch_gemm2<EpiResTma, RPX_RES_STAGES>(A, lda, B, ldb, T, D, K, ep, st);
-  }
-#endif
+int residual_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int T, int D, int K, float* h32,
+                  __nv_bfloat16* h16, float* ss, cudaStream_t st) {
   EpiResidual::Params ep{h32, h16, D, ss, T};
-  return encoder_gemm<EpiResidual>(A, lda, B, ldb, T, D, K, ep, st);
+  return launch_gemm<kBlockN, EpiResidual>(A, lda, B, ldb, T, D, K, ep, st);
 }
 
 struct LayerW {
@@ -140,7 +72,7 @@ extern "C" int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num
 struct rpx_encoder {
   rpx_t5_config cfg;
   int inner = 0;
-  int n_parts = 0;      // RMSNorm partial sums per row on the throughput path: one per 256-wide n-tile
+  int n_parts = 0;      // RMSNorm partial sums per row on the throughput path: one per 128-wide n-tile
   int n_parts_lat = 0;  // ... on the latency path: one per 32-column chunk
   int latency_tokens = 0;  // calls with at most this many packed tokens take the latency path (0: never)
   size_t layer_bytes = 0;  // packed weights of one layer (qkv | o | wi | wo, contiguous from LayerW::qkv)
@@ -289,28 +221,27 @@ struct Prof {
 
 // ---------------------------------------------------------------------------------------------
 // Latency path: one proof state per call (`retrieve`, retrieval/model.py:348-357, encodes ONE context).
-// With T of a few hundred tokens the 256 x 256 pair tiles of the throughput path leave most of the GPU
-// idle (QKV: 5 tiles, O / FFN-down: 6 tiles on 74 pairs) and every GEMM is bound by the latency of
-// streaming its operands through a handful of SMs.  Here the same contraction core runs narrow 1-CTA tiles:
-//   up to 384 tokens   QKV, O-proj, FFN-down on 64-ROW tiles (tcgen05.mma M = 64) x 64 columns with a 12-deep
-//                      ring of 16 KB stages: 72 / 92 CTAs for a 200-token state, 138 at 384 tokens (one wave);
-//                      a narrow GEMM's time is its k-blocks times the round trip of the operand ring divided by
-//                      the ring depth, and half-empty 128-row tiles would cost their full intake
-//   beyond             128 x 64 tiles, 8-deep ring (the 64-row tiles would need a second wave: 512 tokens 0.99
-//                      vs 0.59 ms)
+// With T of a few hundred tokens the 128 x 128 tiles of the throughput path leave most of the GPU idle
+// (QKV: 9 tiles, O / FFN-down: 12 tiles for a 128-token state) and every GEMM is bound by the latency of
+// streaming its operands through a handful of SMs.  Here the same contraction core runs narrow tiles:
+//   up to 384 tokens   QKV, O-proj, FFN-down on 64-ROW tiles (one wgmma row block) x 64 columns with a 12-deep
+//                      ring of 16 KB stages: 6 row tiles x 23 column tiles = 138 CTAs at 384 tokens for
+//                      d_model = 1472; a narrow GEMM's time is its k-blocks times the round trip of the operand
+//                      ring divided by the ring depth, and half-empty 128-row tiles would cost their full intake
+//   beyond             128 x 64 tiles, 6-deep ring (what fits beside the 34 KB accumulator tile)
 //   FFN-up             128 x 128 tiles = 64 gated hidden units (128 x 64 = 32 units up to 128 tokens), B tile in
 //                      two boxes (gate rows, linear rows)
 // K is never split, so every output element is accumulated over k in the same order whatever the tile, and
 // the residual epilogues write their RMSNorm partial sums per 32-column chunk (n_parts_lat of them) whatever
 // the tile: a state's embedding does not depend on what it was batched with.
 constexpr int kLatBlockN = 64;
-constexpr int kLatStages = 8;
+constexpr int kLatStages = 6;
 constexpr int kLatSmallM = 64;
 constexpr int kLatSmallStages = 12;
-constexpr int kLatSmallMMaxTokens = 384;  // 6 row tiles x 23 column tiles = 138 CTAs: the most one wave holds
-// Calls of at most this many tokens run their kernel chain under programmatic dependent launch: at 4 k tokens
-// the re-indexing tiles gain 7 % (2.03 -> 1.89 ms), at 16 k 3-8 %, from 32 k on it is neutral to -1 % (A/B,
-// BASELINE config-5 rows, two runs each).
+constexpr int kLatSmallMMaxTokens = 384;
+// Calls of at most this many tokens run their kernel chain under programmatic dependent launch: it hides
+// the prologue of each kernel behind the tail of its predecessor, which matters while the tails are a
+// noticeable share of a kernel's time.
 constexpr int kPdlMaxTokens = 16384;
 
 int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, const void* next_weights,
@@ -321,8 +252,8 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   {
     Prof p(e, st, 1);
     EpiStoreBF16::Params ep{ws.qkv, 3 * inner, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}};
-    // the QKV projection occupies 18 x ceil(T/64) (or 18 x ceil(T/128)) SMs: the rest of the GPU fetches the
-    // next layer's weights into L2
+    // the QKV projection occupies 18 x ceil(T/64) (or 18 x ceil(T/128)) SMs for 6 heads: the rest of the GPU
+    // fetches the next layer's weights into L2
     if (T <= kLatSmallMMaxTokens) {
       RPX_TRY((launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(ws.h16, D, w.qkv, D, T, 3 * inner,
                                                                                                  D, ep, st, 0, next_weights,
@@ -335,7 +266,7 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   {
     Prof p(e, st, 2);
     RPX_TRY(launch_t5_attention(ws.qkv, ws.attn, ws.cu_tokens, e->bias_lut, T, S, max_len, c.num_heads, c.d_kv,
-                                c.rel_max_distance, st, true));
+                                c.rel_max_distance, st));
   }
   {
     Prof p(e, st, 3);
@@ -355,7 +286,7 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
       RPX_TRY((launch_gemm<64, EpiGeGLUT<32>, false, kLatStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
     } else {
       EpiGeGLUT<64>::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((launch_gemm<128, EpiGeGLUT<64>, false, 6, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
+      RPX_TRY((launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
     }
   }
   {
@@ -395,8 +326,6 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     return RPX_OK;
   };
   RPX_TRY(dump(0));
-  ResidualMaps maps;
-  if (!latency) RPX_TRY(make_residual_maps(&maps, ws.h32, ws.h16, T, D));
   for (int l = 0; l < c.num_layers; ++l) {
     const LayerW& w = e->layers[l];
     if (latency) {
@@ -409,7 +338,7 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     {
       Prof p(e, st, 1);
       EpiStoreBF16::Params ep{ws.qkv, 3 * inner, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((encoder_gemm<EpiStoreBF16>(ws.h16, D, w.qkv, D, T, 3 * inner, D, ep, st)));
+      RPX_TRY((launch_gemm<kBlockN, EpiStoreBF16>(ws.h16, D, w.qkv, D, T, 3 * inner, D, ep, st)));
     }
     {
       Prof p(e, st, 2);
@@ -418,16 +347,16 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     }
     {
       Prof p(e, st, 3);
-      RPX_TRY(residual_gemm(maps, ws.attn, inner, w.o, inner, T, D, inner, ws.h32, ws.h16, ws.ssB, st));
+      RPX_TRY(residual_gemm(ws.attn, inner, w.o, inner, T, D, inner, ws.h32, ws.h16, ws.ssB, st));
     }
     {
       Prof p(e, st, 4);
-      EpiGeGLU::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((encoder_gemm<EpiGeGLU>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
+      EpiGeGLUT<kBlockN / 2>::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
+      RPX_TRY((launch_gemm<kBlockN, EpiGeGLUT<kBlockN / 2>, false, kGemmStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
     }
     {
       Prof p(e, st, 5);
-      RPX_TRY(residual_gemm(maps, ws.ffn, F, w.wo, F, T, D, F, ws.h32, ws.h16, ws.ssA, st));
+      RPX_TRY(residual_gemm(ws.ffn, F, w.wo, F, T, D, F, ws.h32, ws.h16, ws.ssA, st));
     }
     RPX_TRY(dump(l + 1));
   }

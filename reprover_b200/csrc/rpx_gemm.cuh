@@ -1,19 +1,20 @@
-// rpx_gemm.cuh — the tcgen05 / TMA / TMEM contraction core shared by the encoder
-// GEMMs and the similarity kernel.
+// rpx_gemm.cuh — the wgmma / TMA contraction core shared by the encoder GEMMs and the
+// similarity kernel.
 //
-//   D[M, N] (fp32, in TMEM) = A[M, K] * B[N, K]^T        A, B bf16, K contiguous
+//   D[M, N] (fp32) = A[M, K] * B[N, K]^T        A, B bf16, K contiguous
 //
-// Structure (one persistent CTA per SM, 192 threads):
-//   warp 0      : TMA producer   — cp.async.bulk.tensor A/B tiles into a STAGES-deep
+// Structure (one persistent CTA per SM, 160 + 32 * Epi::kWarps threads):
+//   warps 0-3   : MMA warpgroup  — wgmma.mma_async (M = 64 per instruction, one instruction per
+//                 64-row half of the tile, N = BLOCK_N, K = 16) x4 per stage, the fp32 accumulator in
+//                 registers; a stage goes back to the producer (`empty[]`) once the wgmma group that read
+//                 it has retired.  After the last k-block the accumulator is written to a shared-memory
+//                 tile (`acc`, one row of BLOCK_N floats per output row) and published (`tfull`).
+//   warp 4      : TMA producer   — cp.async.bulk.tensor A/B tiles into a STAGES-deep
 //                 128B-swizzled shared-memory ring, completion on `full[]` mbarriers
-//   warp 1      : MMA issuer     — one elected thread issues tcgen05.mma (M=128,
-//                 N<=256, K=16) x4 per stage; tcgen05.commit releases the stage
-//                 (`empty[]`) and, after the last k-block, publishes the accumulator
-//                 (`tfull[]`).  Also owns TMEM alloc/dealloc.
-//   warps 2..5  : epilogue       — tcgen05.ld the accumulator (one row per thread)
-//                 and run the fused epilogue functor; `tempty[]` hands the TMEM
-//                 stage back.  Two accumulator stages (2 x BLOCK_N columns) let the
-//                 epilogue of tile i overlap the mainloop of tile i+1.
+//   warps 5..   : epilogue       — read the accumulator tile (one row per thread) and run the fused
+//                 epilogue functor; `tempty` hands the tile back.  The MMA warpgroup runs the mainloop of
+//                 tile i+1 while the epilogue works on tile i; it only waits for `tempty` before it writes
+//                 the next accumulator.
 //
 // `n_blk_stride` > 1 makes the kernel visit only every stride-th B tile (the similarity
 // kernel's sampling pass); it is 1 everywhere else.
@@ -33,29 +34,33 @@ namespace rpx {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle atom row
-constexpr int kUmmaK = 16;
+constexpr int kMmaK = 16;
 #ifndef RPX_EPI_WARPS
 #define RPX_EPI_WARPS 4
 #endif
-constexpr int kEpiWarp0 = 2;  // first epilogue warp
-// threads of a launch: TMA warp + MMA warp + Epi::kWarps epilogue warps (4 or 8)
+constexpr int kMmaThreads = 128;  // warps 0-3: the MMA warpgroup
+constexpr int kProducerWarp = 4;
+constexpr int kEpiWarp0 = 5;      // first epilogue warp
+// threads of a launch: MMA warpgroup + TMA warp + Epi::kWarps epilogue warps (4 or 8)
 template <class Epi>
-constexpr int gemm_threads() { return 64 + 32 * Epi::kWarps; }
+constexpr int gemm_threads() { return kMmaThreads + 32 + 32 * Epi::kWarps; }
 
 template <int BLOCK_N, int STAGES, int BM = kBlockM>
 struct GemmCfg {
-  static_assert(BM == 64 || BM == 128, "UMMA M of a 1-CTA tile: 64 or 128");
-  static_assert(2 * STAGES + 4 <= 30, "barrier block holds at most 13 stages");
+  static_assert(BM == 64 || BM == 128, "tile rows: one or two 64-row wgmma blocks");
+  static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma N of a tile: 64 or 128");
+  static_assert(2 * STAGES + 2 <= 30, "barrier block holds at most 14 stages");
   static constexpr int kABytes = BM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 2 * BLOCK_N;  // two accumulator stages
-  static_assert(kTmemCols == 64 || kTmemCols == 128 || kTmemCols == 256 || kTmemCols == 512,
-                "TMEM allocation must be a power of two in [32, 512]");
-  // ring + 1 KB alignment slack + barriers/tmem pointer
+  // accumulator tile: BM rows of BLOCK_N floats, rows padded by 4 floats so that the eight rows a
+  // quarter-warp reads at once (16 B each) fall into distinct banks
+  static constexpr int kAccStride = BLOCK_N + 4;
+  static constexpr int kAccBytes = BM * kAccStride * 4;
+  // ring + accumulator + 1 KB alignment slack + barriers
   static constexpr int kBarBytes = 256;
   static constexpr size_t smem_bytes(size_t epi_extra) {
-    return (size_t)STAGES * kStageBytes + 1024 + kBarBytes + epi_extra;
+    return (size_t)STAGES * kStageBytes + kAccBytes + 1024 + kBarBytes + epi_extra;
   }
 };
 
@@ -80,7 +85,7 @@ RPX_DEVICE unsigned long long global_ns() {
 
 // What an epilogue functor sees for one output tile.
 struct TileCtx {
-  uint32_t tmem;   // TMEM address of this thread's row, column 0 of the accumulator stage
+  const float* acc;  // this thread's row of the accumulator tile (shared memory), column 0
   int m0, n0;      // tile origin in the output
   int n_cols;      // valid columns in this tile (multiple of 32)
   int row;         // this thread's row inside the tile, 0..127
@@ -89,41 +94,62 @@ struct TileCtx {
   int next_m0, next_n0;  // origin of the next tile this CTA will process (next_m0 < 0: none)
   int next_cols;         // its width
   int part, split;       // this warp handles the 32-column chunks with (chunk % split) == part
-  int rows_per_warp;     // tile rows held by one TMEM lane group: 32 (M = 128 tiles) or 16 (M = 64: lanes 16-31 idle)
+  int rows_per_warp;     // tile rows held by one lane group: 32 (M = 128 tiles) or 16 (M = 64: lanes 16-31 idle)
 };
+
+// 32 consecutive accumulator columns of this thread's row.
+RPX_DEVICE void acc_ld32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 x = reinterpret_cast<const float4*>(src)[i];
+    v[4 * i] = __float_as_uint(x.x);
+    v[4 * i + 1] = __float_as_uint(x.y);
+    v[4 * i + 2] = __float_as_uint(x.z);
+    v[4 * i + 3] = __float_as_uint(x.w);
+  }
+}
 
 // Epi must provide:
 //   struct Params;                       (trivially copyable kernel argument)
 //   static constexpr size_t kSmemBytes;  (extra dynamic shared memory, may be 0)
-//   static constexpr int kWarps;         (4 or 8 epilogue warps; with 8, two warps share a TMEM lane
+//   static constexpr int kWarps;         (4 or 8 epilogue warps; with 8, two warps share a lane
 //                                         group and split the tile's 32-column chunks between them)
 //   __device__ Epi(const Params&, uint8_t* smem_extra, int row /*tile row this thread owns, 0..127*/,
 //                  int part /*column share of this warp, 0..kWarps/4-1*/);
 //   __device__ void before_wait(const TileCtx&);  (work that may run while the MMAs of this tile are
 //                                                  still in flight, e.g. prefetching)
-//   __device__ void tile(const TileCtx&);     (all 128 epilogue threads, warp-converged)
+//   __device__ void tile(const TileCtx&);     (all epilogue threads, warp-converged)
 //   __device__ void finish();
-// SPLIT_B (the gated FFN up-projection on narrow tiles): the B tile is two boxes of BLOCK_N/2 rows — the
-// gate rows and the linear-branch rows of the same BLOCK_N/2 hidden units.  The packed weight interleaves
-// wi_0 / wi_1 in 128-row blocks (rows [256j, 256j+128) gate, [256j+128, 256j+256) linear, see
-// rpx_encoder.cu), so n-tile t (units u0 = t * BLOCK_N/2) takes rows 256 (u0/128) + u0 % 128 and the same + 128;
-// tmB must then be encoded with a box of BLOCK_N/2 rows.
+// SPLIT_B (the gated FFN up-projection): the B tile is two boxes of BLOCK_N/2 rows — the gate rows and the
+// linear-branch rows of the same BLOCK_N/2 hidden units.  The packed weight interleaves wi_0 / wi_1 in
+// 128-row blocks (rows [256j, 256j+128) gate, [256j+128, 256j+256) linear, see rpx_encoder.cu), so n-tile t
+// (units u0 = t * BLOCK_N/2) takes rows 256 (u0/128) + u0 % 128 and the same + 128; tmB must then be encoded
+// with a box of BLOCK_N/2 rows.
 //
-// BM = 64 (latency path): 64-row tiles, tcgen05.mma M = 64.  The accumulator then occupies lanes 0-15 of each
-// 32-lane TMEM group (row r of the tile sits in lane 32 (r / 16) + r % 16), so an epilogue warp owns 16 rows and
-// its upper 16 lanes idle.  A CTA takes in half the activation bytes per k-block and the ring holds more
-// stages — what a narrow GEMM's time is made of (see rpx_encoder.cu).
-template <int BLOCK_N, int STAGES, class Epi, bool M_FASTEST = false, bool SPLIT_B = false, int BM = kBlockM>
+// PAIR: the kernel runs as clusters of two CTAs that work in lockstep on vertically adjacent tiles — the same
+// n-tile, m-tiles 2j and 2j+1 — and share the B tile: each CTA's producer loads one half of it (BLOCK_N/2 rows,
+// tmB encoded with that box) and multicasts it into both CTAs, so every B byte crosses L2 once per pair.  A
+// stage is refilled only after the MMA warpgroups of BOTH CTAs have released it (the empty barriers count the
+// peer's arrivals too), since the refill writes into the peer's shared memory as well.  Grid = 2 x pairs.
+//
+// BM = 64 (latency path): 64-row tiles, one wgmma row block.  An epilogue warp then owns 16 rows (row r of the
+// tile belongs to lane r % 16 of lane group r / 16) and its upper 16 lanes idle.  A CTA takes in half the
+// activation bytes per k-block and the ring holds more stages — what a narrow GEMM's time is made of (see
+// rpx_encoder.cu).
+template <int BLOCK_N, int STAGES, class Epi, bool M_FASTEST = false, bool SPLIT_B = false, int BM = kBlockM,
+          bool PAIR = false>
 __global__ void __launch_bounds__(gemm_threads<Epi>(), 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                int M, int N, int K, int tiles_m, int tiles_n, int n_blk_stride, typename Epi::Params ep,
                L2Prefetch pf) {
   using Cfg = GemmCfg<BLOCK_N, STAGES, BM>;
+  constexpr int kSub = BM / 64;  // 64-row wgmma blocks per tile
+  static_assert(!PAIR || (!M_FASTEST && !SPLIT_B), "paired tiles: plain n-fastest order, one B box per CTA");
   if (threadIdx.x == 0) RPX_STAMP(pf, 0);
   if ((int)blockIdx.x >= pf.work_ctas) {
     // Helper CTA (latency path): the GEMM itself keeps only a fraction of the SMs busy, so the launch is
-    // widened to the whole GPU and the surplus CTAs pull the NEXT layer's weights into L2 (36 MB of 126 MB)
-    // while this layer computes — its GEMMs then stream their B operand at L2 instead of DRAM latency.
+    // widened to the whole GPU and the surplus CTAs pull the NEXT layer's weights into L2 while this
+    // layer computes — its GEMMs then stream their B operand at L2 instead of DRAM latency.
     pdl_launch_dependents();
     const int n_help = (int)gridDim.x - pf.work_ctas;
     const size_t lines = ((size_t)pf.bytes + 127) >> 7;
@@ -139,50 +165,49 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = smem_raw + ((1024 - (raw_addr & 1023)) & 1023);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * Cfg::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::kStageBytes);
+  float* sAcc = reinterpret_cast<float*>(smem + STAGES * Cfg::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::kStageBytes + Cfg::kAccBytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + STAGES;
   uint64_t* tfull = bars + 2 * STAGES;
-  uint64_t* tempty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint8_t* smem_extra = smem + STAGES * Cfg::kStageBytes + Cfg::kBarBytes;
+  uint64_t* tempty = bars + 2 * STAGES + 1;
+  uint8_t* smem_extra = smem + STAGES * Cfg::kStageBytes + Cfg::kAccBytes + Cfg::kBarBytes;
 
   const int warp = threadIdx.x >> 5;
-  const int num_tiles = tiles_m * tiles_n;
   const int num_kb = K / kBlockK;
+  // Work units: tiles, or (PAIR) tile pairs; this CTA takes units unit0, unit0 + unit_step, ...
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
+  const int num_units = PAIR ? ((tiles_m + 1) / 2) * tiles_n : tiles_m * tiles_n;
+  const int unit0 = PAIR ? (int)blockIdx.x >> 1 : (int)blockIdx.x;
+  const int unit_step = PAIR ? pf.work_ctas >> 1 : pf.work_ctas;
+  auto unit_m = [&](int u) { return PAIR ? 2 * (u / tiles_n) + (int)rank : (M_FASTEST ? u % tiles_m : u / tiles_n); };
+  auto unit_n = [&](int u) { return PAIR ? u % tiles_n : (M_FASTEST ? u / tiles_m : u % tiles_n); };
 
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) {
+  if (warp == kProducerWarp) {
     if (elect_one()) {
+      tma_prefetch_desc(&tmA);
+      tma_prefetch_desc(&tmB);
       for (int s = 0; s < STAGES; ++s) {
         mbar_init(&full[s], 1);
-        mbar_init(&empty[s], 1);
+        mbar_init(&empty[s], PAIR ? 2 * kMmaThreads : kMmaThreads);
       }
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(&tfull[s], 1);
-        mbar_init(&tempty[s], 32 * Epi::kWarps);
-      }
+      mbar_init(tfull, kMmaThreads);
+      mbar_init(tempty, 32 * Epi::kWarps);
       fence_mbar_init();
     }
     __syncwarp();
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Everything above touched only this CTA's shared memory / TMEM.  Under programmatic dependent launch
+  if (PAIR) cluster_sync_all();  // the peer's barriers are initialised before anything multicasts or arrives on them
+  // Everything above touched only this CTA's shared memory.  Under programmatic dependent launch
   // (rpx_ptx.cuh) the preceding kernel may still be running: the A operand and whatever the epilogue reads
   // from global memory are its outputs and must wait for it (pdl_wait), but the B operand — the weights —
   // is never written by a kernel of the chain, so the producer streams the first ring's worth of B tiles
-  // BEFORE it waits: by the time the predecessor retires, a third of this CTA's weights are already on chip.
+  // BEFORE it waits: by the time the predecessor retires, part of this CTA's weights are already on chip.
   pdl_launch_dependents();
   if (threadIdx.x == 0) RPX_STAMP(pf, 1);
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------------ TMA producer
     if (elect_one()) {
       int stage = 0;
@@ -191,6 +216,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       auto load_b = [&](int st, int n_blk, int kb) {
         if (M_FASTEST) {
           tma_load_2d_hint(sB + st * Cfg::kBBytes, &tmB, &full[st], kb * kBlockK, n_blk * n_blk_stride * BLOCK_N, kEvictFirst);
+        } else if (PAIR) {
+          constexpr int H = BLOCK_N / 2;
+          tma_load_2d_multicast(sB + st * Cfg::kBBytes + rank * H * kBlockK * 2, &tmB, &full[st], kb * kBlockK,
+                                n_blk * BLOCK_N + (int)rank * H, (uint16_t)0x3);
         } else if (SPLIT_B) {
           constexpr int H = BLOCK_N / 2;
           const int u0 = n_blk * H;
@@ -201,8 +230,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           tma_load_2d(sB + st * Cfg::kBBytes, &tmB, &full[st], kb * kBlockK, n_blk * n_blk_stride * BLOCK_N);
         }
       };
-      if (!M_FASTEST && (int)blockIdx.x < num_tiles) {
-        const int n_blk0 = (int)blockIdx.x % tiles_n;
+      if (!M_FASTEST && !PAIR && unit0 < num_units) {
+        const int n_blk0 = unit_n(unit0);
         pre = num_kb < STAGES ? num_kb : STAGES;
         for (int kb = 0; kb < pre; ++kb) {  // fresh barriers: every stage is free
           mbar_arrive_expect_tx(&full[kb], Cfg::kStageBytes);
@@ -211,22 +240,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       pdl_wait();
       RPX_STAMP(pf, 2);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += pf.work_ctas) {
-        const int n_blk = M_FASTEST ? tile / tiles_m : tile % tiles_n;
-        const int m_blk = M_FASTEST ? tile % tiles_m : tile / tiles_n;
+      for (int u = unit0; u < num_units; u += unit_step) {
+        const int n_blk = unit_n(u);
+        const int m_blk = unit_m(u);
         for (int kb = 0; kb < num_kb; ++kb) {
           if (pre > 0) {
             --pre;  // armed, B in flight: only the A tile is missing
           } else {
-            mbar_wait(&empty[stage], phase ^ 1, 1);
+            mbar_wait(&empty[stage], phase ^ 1);
             mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
             load_b(stage, n_blk, kb);
           }
-          // L2 eviction hints: streamed operand evict-first, re-used operand evict-last.  Measured
-          // on B200 (A/B, one box): -20 % time for the similarity kernel (corpus streamed once, query
-          // block re-read by every tile), +3 % for the encoder GEMMs -> M_FASTEST only.  (An L2
-          // prefetch of the streamed operand a few k-blocks ahead of its TMA load was also measured:
-          // 6-12 % slower at every distance tried, removed.)
+          // L2 eviction hints for the similarity kernel: the streamed operand (corpus) evict-first, the
+          // re-used operand (query block, re-read by every tile) evict-last.
           if (M_FASTEST) {
             tma_load_2d_hint(sA + stage * Cfg::kABytes, &tmA, &full[stage], kb * kBlockK, m_blk * BM, kEvictLast);
           } else {
@@ -239,61 +265,86 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += pf.work_ctas) {
-        const int n_blk = M_FASTEST ? tile / tiles_m : tile % tiles_n;
-        int n_this = N - n_blk * n_blk_stride * BLOCK_N;
-        if (n_this > BLOCK_N) n_this = BLOCK_N;
-        n_this = (n_this + 15) & ~15;
-        const uint32_t idesc = make_idesc_bf16(BM, (uint32_t)n_this);
-        mbar_wait(&tempty[as], aphase ^ 1, 2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase, 3);
-          if (kb == 0 && tile == (int)blockIdx.x) RPX_STAMP(pf, 3);
-          tc_fence_after();
-          const uint64_t a_desc = make_smem_desc_kmajor_sw128(smem_u32(sA + stage * Cfg::kABytes));
-          const uint64_t b_desc = make_smem_desc_kmajor_sw128(smem_u32(sB + stage * Cfg::kBBytes));
+  } else if (warp < kProducerWarp) {
+    // ------------------------------------------------------------------ MMA warpgroup
+    const int lane = threadIdx.x & 31;
+    float acc[kSub][BLOCK_N / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t tphase = 0;
+    auto release = [&](int st) {
+      mbar_arrive(&empty[st]);
+      if (PAIR) mbar_arrive_cluster(&empty[st], rank ^ 1u);
+    };
+    for (int u = unit0; u < num_units; u += unit_step) {
+      int prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        if (kb == 0 && u == unit0 && threadIdx.x == 0) RPX_STAMP(pf, 3);
+        const uint64_t a_desc = make_smem_desc_kmajor_sw128(smem_u32(sA + stage * Cfg::kABytes));
+        const uint64_t b_desc = make_smem_desc_kmajor_sw128(smem_u32(sB + stage * Cfg::kBBytes));
 #pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            // +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom
-            umma_bf16_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (kb | k) != 0);
-          }
-          umma_commit(&empty[stage]);
-          if (kb == num_kb - 1 && tile == (int)blockIdx.x) RPX_STAMP(pf, 4);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
+        for (int s = 0; s < kSub; ++s) wgmma_fence_operand(acc[s]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kMmaK; ++k) {
+#pragma unroll
+          for (int s = 0; s < kSub; ++s) {
+            // +32 bytes (>>4 = 2) per K=16 step inside the swizzle atom; +8 KB (>>4 = 512) per 64 A rows
+            if constexpr (BLOCK_N == 128)
+              wgmma_m64n128k16_ss(acc[s], a_desc + 512 * s + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+            else
+              wgmma_m64n64k16_ss(acc[s], a_desc + 512 * s + 2 * k, b_desc + 2 * k, (kb | k) != 0);
           }
         }
-        umma_commit(&tfull[as]);
-        as ^= 1;
-        if (as == 0) aphase ^= 1;
+        wgmma_commit();
+        // the group of the previous k-block has retired once at most this one is in flight: its stage is free
+        if (kb > 0) {
+          wgmma_wait<1>();
+          release(prev);
+        }
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
       }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int s = 0; s < kSub; ++s) wgmma_fence_operand(acc[s]);
+      release(prev);
+      if (u == unit0 && threadIdx.x == 0) RPX_STAMP(pf, 4);
+      // accumulator -> shared memory, once the epilogue has finished reading the previous tile
+      mbar_wait(tempty, tphase ^ 1);
+      const int r0 = (warp * 16 + (lane >> 2)) * Cfg::kAccStride + 2 * (lane & 3);
+#pragma unroll
+      for (int s = 0; s < kSub; ++s) {
+        float* dst = sAcc + s * 64 * Cfg::kAccStride + r0;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[s][4 * j], acc[s][4 * j + 1]);
+          *reinterpret_cast<float2*>(dst + 8 * Cfg::kAccStride + 8 * j) = make_float2(acc[s][4 * j + 2], acc[s][4 * j + 3]);
+        }
+      }
+      mbar_arrive(tfull);
+      tphase ^= 1;
     }
   } else {
     // ------------------------------------------------------------------ epilogue
-    const int lane_grp = warp & 3;                            // TMEM lane group this warp may read
+    const int lane_grp = (warp - kEpiWarp0) & 3;              // which 32 (or 16) rows of the tile
     const int lane = threadIdx.x & 31;
     // row of the tile this thread owns; with 64-row tiles lanes 16-31 of a group hold nothing: their row lies
-    // beyond every matrix, so the functors' `m < M` tests switch them off
+    // beyond every matrix, so the functors' `m < M` tests switch them off (they read a duplicate row)
     const int row = BM == kBlockM ? lane_grp * 32 + lane : (lane < 16 ? lane_grp * 16 + lane : (1 << 28));
+    const int acc_row = BM == kBlockM ? lane_grp * 32 + lane : lane_grp * 16 + (lane & 15);
     const int part = (warp - kEpiWarp0) >> 2;                 // which share of the columns (0 when 4 warps)
     pdl_wait();  // the epilogue reads (row scales, residual stream) and overwrites the predecessor's outputs
-    Epi epi(ep, smem_extra, lane_grp * 32 + lane, part);      // (the functor's staging is per TMEM lane)
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += pf.work_ctas) {
+    Epi epi(ep, smem_extra, lane_grp * 32 + lane, part);      // (the functor's staging is per lane group)
+    uint32_t tphase = 0;
+    for (int u = unit0; u < num_units; u += unit_step) {
       TileCtx t;
-      t.n_blk = M_FASTEST ? tile / tiles_m : tile % tiles_n;
-      t.m_blk = M_FASTEST ? tile % tiles_m : tile / tiles_n;
+      t.n_blk = unit_n(u);
+      t.m_blk = unit_m(u);
       t.m0 = t.m_blk * BM;
       t.rows_per_warp = BM / 4;
       t.n0 = t.n_blk * n_blk_stride * BLOCK_N;  // (n_blk stays the logical tile index)
@@ -305,12 +356,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       t.split = Epi::kWarps / 4;
       t.M = M;
       t.N = N;
-      t.tmem = tmem_base + as * BLOCK_N + ((uint32_t)(lane_grp * 32) << 16);
+      t.acc = sAcc + acc_row * Cfg::kAccStride;
       {
-        const int nt = tile + pf.work_ctas;
-        if (nt < num_tiles) {
-          t.next_m0 = (M_FASTEST ? nt % tiles_m : nt / tiles_n) * BM;
-          t.next_n0 = (M_FASTEST ? nt / tiles_m : nt % tiles_n) * BLOCK_N;
+        const int nu = u + unit_step;
+        if (nu < num_units) {
+          t.next_m0 = unit_m(nu) * BM;
+          t.next_n0 = unit_n(nu) * BLOCK_N;
           t.next_cols = N - t.next_n0 < BLOCK_N ? N - t.next_n0 : BLOCK_N;
         } else {
           t.next_m0 = -1;
@@ -319,25 +370,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
       epi.before_wait(t);
-      mbar_wait(&tfull[as], aphase, 4);
-      if (threadIdx.x == 64 && tile == (int)blockIdx.x) RPX_STAMP(pf, 5);
-      tc_fence_after();
+      mbar_wait(tfull, tphase);
+      if (threadIdx.x == 32 * kEpiWarp0 && u == unit0) RPX_STAMP(pf, 5);
       epi.tile(t);
-      if (threadIdx.x == 64 && tile == (int)blockIdx.x) RPX_STAMP(pf, 6);
-      tc_fence_before();
-      mbar_arrive(&tempty[as]);
-      as ^= 1;
-      if (as == 0) aphase ^= 1;
+      if (threadIdx.x == 32 * kEpiWarp0 && u == unit0) RPX_STAMP(pf, 6);
+      mbar_arrive(tempty);
+      tphase ^= 1;
     }
     epi.finish();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
+  // the peer may still multicast into this CTA's ring or arrive on its barriers until it is done too
+  if (PAIR) cluster_sync_all();
   if (threadIdx.x == 0) RPX_STAMP(pf, 7);
 }
 
@@ -388,8 +433,7 @@ struct EpiStoreF32 {
     const bool ok = m < t.M;
     for (int c = 32 * t.part; c < t.n_cols; c += 32 * t.split) {
       uint32_t v[32];
-      tmem_ld_32x32(t.tmem + c, v);
-      tmem_ld_wait();
+      acc_ld32(t.acc + c, v);
       if (ok) {
         float4* dst = reinterpret_cast<float4*>(p.C + (size_t)m * p.ldc + t.n0 + c);
 #pragma unroll
@@ -425,8 +469,7 @@ struct EpiStoreBF16 {
     const bool ok = m < t.M;
     for (int c = 32 * t.part; c < t.n_cols; c += 32 * t.split) {
       uint32_t v[32];
-      tmem_ld_32x32(t.tmem + c, v);
-      tmem_ld_wait();
+      acc_ld32(t.acc + c, v);
       if (ok) {
         uint4* dst = reinterpret_cast<uint4*>(p.C + (size_t)m * p.ldc + t.n0 + c);
 #pragma unroll
@@ -449,16 +492,12 @@ struct EpiStoreBF16 {
 // The fp32 copy is the residual stream; the bf16 copy is the next GEMM's A operand;
 // ss_out feeds the next RMSNorm (see RowScale).
 //
-// The accumulator arrives one ROW per thread (TMEM lane == thread), which is the worst
-// possible layout for global memory: a warp-wide 16-byte access would touch 32 different
-// 128-byte lines.  Each warp therefore transposes its 32x32 fp32 block through a swizzled
-// shared-memory tile and does the read-modify-write with lanes running along the row:
-// one instruction covers 4 rows x 128 contiguous bytes (4 L1 wavefronts instead of 32).
-// Residual loads run one chunk ahead.  (RPX_EPI_WARPS=8 — two warps per TMEM lane group splitting
-// the chunks — was measured neutral to slightly negative on B200 and is off by default.  Measured
-// and dropped: an L2 prefetch of the next tile's residual rows one tile ahead — the lines
-// were evicted again before use, 6.0 GB read per launch against 3.4 GB algorithmic — and L2
-// eviction-priority hints on the residual loads / stores, 0 %.)
+// The accumulator arrives one ROW per thread, which is the worst possible layout for global
+// memory: a warp-wide 16-byte access would touch 32 different 128-byte lines.  Each warp
+// therefore transposes its 32x32 fp32 block through a swizzled shared-memory tile and does the
+// read-modify-write with lanes running along the row: one instruction covers 4 rows x 128
+// contiguous bytes (4 L1 wavefronts instead of 32).  Residual loads run one chunk ahead.
+// (RPX_EPI_WARPS=8 — two warps per lane group splitting the chunks — is off by default.)
 // CHUNK_SS: one partial sum per 32-column chunk instead of one per tile (ss_out is then indexed by the chunk's
 // position in the row, [N / 32][ss_stride]) — the latency path uses 32- or 64-wide tiles depending on the token
 // count and must hand the next RMSNorm the same partial sums either way.
@@ -512,11 +551,10 @@ struct EpiResidualT {
     int c = 32 * t.part;
     for (; c < t.n_cols; c += step) {
       uint32_t v[32];
-      tmem_ld_32x32(t.tmem + c, v);
+      acc_ld32(t.acc + c, v);
       // next chunk's residual loads go out before this chunk is consumed
       if (c + step < t.n_cols) load_chunk(t, c + step, row_base, sub, col4, hn);
       const size_t col = (size_t)t.n0 + c + col4;
-      tmem_ld_wait();
 #pragma unroll
       for (int j = 0; j < 8; ++j)
         stg[lane * 8 + (j ^ (lane & 7))] =
@@ -566,125 +604,6 @@ struct EpiResidualT {
 };
 using EpiResidual = EpiResidualT<false>;
 
-// The same residual update with the data movement handed to the TMA engine (2-CTA kernel only).
-//
-// Why: with K = 384 (attention output projection) the MMA of a tile takes ~2 us while its
-// epilogue has to move 320 KB per CTA; four warps issuing their own loads keep only ~16 KB in
-// flight per SM, and ncu's stall samples sat on the first use of the looked-ahead residual
-// registers (the kernel ran at ~3.2 TB/s inside the step).  Here each epilogue warp owns a ring
-// of R 32x32 fp32 boxes in shared memory: one lane keeps R-1 box loads in flight (across tile
-// boundaries — the next tile's coordinates are known), the warp updates a box in place, row per
-// thread (TMEM lane == thread == box row, 128-byte swizzle => conflict-free 16-byte accesses),
-// and the fp32 box plus its bf16 copy leave again as two bulk tensor stores.  No thread ever
-// waits on a global load or store; rows past M are zero-filled on load and clipped on store.
-template <int R>
-struct EpiResidualTma {
-  struct alignas(64) Params {
-    CUtensorMap tm_h32;  // fp32 [M, N], box 32 cols x 32 rows, 128-byte swizzle (load + store)
-    CUtensorMap tm_h16;  // bf16 [M, N], box 32 cols x 32 rows,  64-byte swizzle (store)
-    float* ss_out;       // [tiles_n][ss_stride]
-    int ss_stride;
-  };
-  static constexpr int kWarps = 4;
-  static constexpr int kInBytes = 32 * 32 * 4;
-  static constexpr int kOutBytes = 32 * 32 * 2;
-  static constexpr int kWarpBytes = R * kInBytes + 2 * kOutBytes;
-  static constexpr size_t kSmemBytes = 1024 + (size_t)kWarps * kWarpBytes + 256;
-  const Params* pp;
-  uint8_t* in;     // this warp's ring
-  uint8_t* out16;  // this warp's two bf16 staging boxes
-  uint64_t* full;  // this warp's R "box landed" barriers
-  int lane, grp;
-  uint32_t seq = 0;  // boxes consumed so far (ring slot = seq % R, parity = (seq / R) & 1)
-  bool primed = false;
-
-  __device__ EpiResidualTma(const Params& p_, uint8_t* smem_extra, int row, int /*part*/) : pp(&p_) {
-    lane = row & 31;
-    grp = row >> 5;
-    uint8_t* base = smem_extra + ((1024 - (smem_u32(smem_extra) & 1023)) & 1023);
-    in = base + grp * kWarpBytes;
-    out16 = in + R * kInBytes;
-    full = reinterpret_cast<uint64_t*>(base + kWarps * kWarpBytes) + grp * R;
-    if (lane == 0) {
-      for (int s = 0; s < R; ++s) mbar_init(&full[s], 1);
-      fence_mbar_init();
-    }
-    __syncwarp();
-  }
-  // Box `idx` counted from the first box of tile t (running on into the next tile) -> ring.
-  __device__ __forceinline__ void issue_load(const TileCtx& t, int idx, uint32_t s) const {
-    const int nch = t.n_cols >> 5;
-    int c0, c1;
-    if (idx < nch) {
-      c0 = t.n0 + 32 * idx;
-      c1 = t.m0 + grp * 32;
-    } else {
-      idx -= nch;
-      if (t.next_m0 < 0 || idx >= (t.next_cols >> 5)) return;
-      c0 = t.next_n0 + 32 * idx;
-      c1 = t.next_m0 + grp * 32;
-    }
-    uint64_t* bar = &full[s % R];
-    mbar_arrive_expect_tx(bar, kInBytes);
-    tma_load_2d(in + (s % R) * kInBytes, &pp->tm_h32, bar, c0, c1);
-  }
-  __device__ void before_wait(const TileCtx& t) {
-    if (primed) return;
-    primed = true;
-    if (lane == 0)
-      for (int k = 0; k < R - 1; ++k) issue_load(t, k, seq + k);
-  }
-  __device__ void tile(const TileCtx& t) {
-    const int nch = t.n_cols >> 5;
-    const int m_w = t.m0 + grp * 32;
-    const int sw = lane & 7;
-    float ss = 0.f;
-    for (int ci = 0; ci < nch; ++ci, ++seq) {
-      const uint32_t slot = seq % R;
-      mbar_wait<0>(&full[slot], (seq / R) & 1, 7);
-      uint32_t v[32];
-      tmem_ld_32x32(t.tmem + 32 * ci, v);
-      tmem_ld_wait();
-      float4* hrow = reinterpret_cast<float4*>(in + slot * kInBytes) + lane * 8;
-      uint4* orow = reinterpret_cast<uint4*>(out16 + (seq & 1) * kOutBytes) + lane * 4;
-      uint32_t pk[16];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 x = hrow[j ^ sw];
-        x.x += __uint_as_float(v[4 * j]);
-        x.y += __uint_as_float(v[4 * j + 1]);
-        x.z += __uint_as_float(v[4 * j + 2]);
-        x.w += __uint_as_float(v[4 * j + 3]);
-        ss += x.x * x.x + x.y * x.y + x.z * x.z + x.w * x.w;
-        hrow[j ^ sw] = x;
-        pk[2 * j] = pack_bf16x2(x.x, x.y);
-        pk[2 * j + 1] = pack_bf16x2(x.z, x.w);
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q)
-        orow[q ^ ((lane >> 1) & 3)] = make_uint4(pk[4 * q], pk[4 * q + 1], pk[4 * q + 2], pk[4 * q + 3]);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_2d(&pp->tm_h32, in + slot * kInBytes, t.n0 + 32 * ci, m_w);
-        tma_store_2d(&pp->tm_h16, out16 + (seq & 1) * kOutBytes, t.n0 + 32 * ci, m_w);
-        bulk_commit_group();
-        // the previous box's stores have drained their shared-memory reads: its ring slot takes the
-        // load R-1 boxes ahead, and its bf16 staging box is free for the next iteration
-        bulk_wait_group_read<1>();
-        issue_load(t, ci + R - 1, seq + R - 1);
-      }
-      __syncwarp();
-    }
-    const int m = m_w + lane;
-    if (m < t.M) pp->ss_out[(size_t)t.n_blk * pp->ss_stride + m] = ss;
-  }
-  __device__ void finish() {
-    if (lane == 0) bulk_wait_group_read<0>();
-    __syncwarp();
-  }
-};
-
 // gelu_new (tanh form) — HF activations.py NewGELUActivation, used by T5 "gated-gelu".
 __device__ __forceinline__ float gelu_new(float x) {
   const float k0 = 0.7978845608028654f;  // sqrt(2/pi)
@@ -720,9 +639,8 @@ struct EpiGeGLUT {
     const bool ok = m < t.M;
     for (int c = 32 * t.part; c < HALF; c += 32 * t.split) {
       uint32_t g[32], u[32];
-      tmem_ld_32x32(t.tmem + c, g);
-      tmem_ld_32x32(t.tmem + HALF + c, u);
-      tmem_ld_wait();
+      acc_ld32(t.acc + c, g);
+      acc_ld32(t.acc + HALF + c, u);
       if (ok) {
         uint4* dst = reinterpret_cast<uint4*>(p.out + (size_t)m * p.ldo + t.n_blk * HALF + c);
 #pragma unroll

@@ -2,7 +2,6 @@
 #pragma once
 #include "rpx_common.cuh"
 #include "rpx_gemm.cuh"
-#include "rpx_gemm2.cuh"
 
 namespace rpx {
 
@@ -49,14 +48,13 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
   return RPX_OK;
 }
 
-
-constexpr int kGemm2Stages = 6;
-
-// 2-CTA (cta_group::2) launcher: 256 x 256 tiles, one CTA pair per tile, persistent over num_sms/2 pairs.
-template <class Epi, int STAGES = kGemm2Stages>
-int launch_gemm2(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
-                 const typename Epi::Params& ep, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg<STAGES>;
+// Paired form (gemm_tc_kernel<..., PAIR>): clusters of two CTAs on vertically adjacent 128 x 128 tiles that
+// share each B tile through TMA multicast; persistent over num_sms / 2 pairs.
+template <class Epi, int STAGES = kGemmStages>
+int launch_gemm_pair(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
+                     const typename Epi::Params& ep, cudaStream_t stream) {
+  constexpr int BLOCK_N = 128;
+  using Cfg = GemmCfg<BLOCK_N, STAGES, kBlockM>;
   RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
   RPX_REQUIRE(K % kBlockK == 0, RPX_ERR_UNSUPPORTED, "gemm: K=%d must be a multiple of %d", K, kBlockK);
   RPX_REQUIRE(N % 32 == 0, RPX_ERR_UNSUPPORTED, "gemm: N=%d must be a multiple of 32", N);
@@ -64,22 +62,34 @@ int launch_gemm2(const void* A, int64_t lda, const void* B, int64_t ldb, int M, 
   RPX_TRY(get_device_info(&dev));
   CUtensorMap tmA, tmB;
   RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, kBlockM));
-  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, Cfg::kBlockN / 2));
-  const int tiles_m = ceil_div(M, kPairM);
-  const int tiles_n = ceil_div(N, Cfg::kBlockN);
+  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, BLOCK_N / 2));
+  const int tiles_m = ceil_div(M, kBlockM);
+  const int tiles_n = ceil_div(N, BLOCK_N);
   const size_t smem = Cfg::smem_bytes(Epi::kSmemBytes);
-  RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm2: needs %zu B smem, device allows %zu", smem,
+  RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu", smem,
               dev.smem_optin);
-  auto kern = gemm_tc2_kernel<STAGES, Epi>;
+  auto kern = gemm_tc_kernel<BLOCK_N, STAGES, Epi, false, false, kBlockM, true>;
   static thread_local int configured_dev = -1;
   if (configured_dev != dev.device) {
     RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured_dev = dev.device;
   }
-  int pairs = tiles_m * tiles_n;
+  int pairs = ceil_div(tiles_m, 2) * tiles_n;
   if (pairs > dev.num_sms / 2) pairs = dev.num_sms / 2;
-  RPX_CUDA_OK(launch_pdl(kern, dim3(2 * pairs), dim3(gemm_threads<Epi>()), smem, stream, pdl_enabled(), tmA, tmB, M, N, K,
-                         tiles_m, tiles_n, ep));
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2 * pairs);
+  cfg.blockDim = dim3(gemm_threads<Epi>());
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = 2;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  RPX_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, tiles_m, tiles_n, 1, ep,
+                                 L2Prefetch{nullptr, 0u, 2 * pairs, next_timeline_slot()}));
   return RPX_OK;
 }
 

@@ -6,7 +6,7 @@
 // bound of the exactness guard); `rpx_index_topk` is `Corpus.get_nearest_premises`' device half
 // (common.py:307-322) and picks one of three paths:
 //     nq <= 2            rpx_smallq.cu   one HBM-bound streaming kernel (the reference's real call: nq = 1)
-//     otherwise          rpx_simtopk.cu  tcgen05 MMA with the top-k fused into the epilogue
+//     otherwise          rpx_simtopk.cu  wgmma with the top-k fused into the epilogue
 //     k > 200 or flagged rpx_exact.cu    exact fp64 pass (always launched; returns at once if idle)
 #include <stdlib.h>
 
@@ -32,10 +32,9 @@ constexpr int kMaxSmsForSizing = 160;  // workspace queries work without a devic
 int small_q_max() {
   static int v = -1;
   if (v < 0) {
-    // Largest nq routed to the streaming kernel (0..4; RPX_SMALLQ_MAX overrides).  Measured on B200, 200k x 1472,
-    // k = 100 (tools/topk_bench.py): nq = 1  0.121 ms streaming vs 0.194 ms tcgen05;  nq = 2  0.162 vs 0.175;
-    // nq = 3 (two passes)  0.280 vs 0.181;  nq = 4  0.260 vs 0.179 (the FMA work of four queries per index
-    // byte is what a tensor core is for).
+    // Largest nq routed to the streaming kernel (0..4; RPX_SMALLQ_MAX overrides, tools/topk_bench.py times every
+    // path by query count).  One or two queries leave the streaming kernel HBM-bound; from three on it needs a
+    // second pass, and the FMA work of several queries per index byte is what a tensor core is for.
     const char* e = getenv("RPX_SMALLQ_MAX");
     v = e ? atoi(e) : 2;
     if (v < 0) v = 0;
@@ -111,7 +110,7 @@ int topk_dispatch(const rpx_index* ix, const void* d_Q, int32_t nq, int32_t k, c
   void* cand_ws = base + L.cand;
   void* path_ws = base + L.path;
 
-  int path = 0;  // 1 tcgen05, 2 streaming, 4 exact
+  int path = 0;  // 1 tensor core, 2 streaming, 4 exact
   if (flags & RPX_TOPK_FORCE_EXACT) path = 4;
   else if (flags & RPX_TOPK_FORCE_STREAM) path = 2;
   else if (flags & RPX_TOPK_FORCE_MMA) path = 1;
@@ -123,7 +122,7 @@ int topk_dispatch(const rpx_index* ix, const void* d_Q, int32_t nq, int32_t k, c
                 "top-k: the streaming path takes 1..4 queries, k <= %d, d <= 2048, n > 0", kFastPathMaxK);
     RPX_TRY(launch_smallq_topk(c, path_ws, topk_n_res(k)));
   } else if (path == 1) {
-    RPX_REQUIRE(k <= kFastPathMaxK, RPX_ERR_UNSUPPORTED, "top-k: the tcgen05 path takes k <= %d", kFastPathMaxK);
+    RPX_REQUIRE(k <= kFastPathMaxK, RPX_ERR_UNSUPPORTED, "top-k: the tensor-core path takes k <= %d", kFastPathMaxK);
     RPX_TRY(run_mma_topk(c, path_ws, workspace_bytes - L.path));
   }
   // exact pass: every query when it is the chosen path, otherwise only what the guard flagged
@@ -179,7 +178,7 @@ int rpx_index_stats(rpx_index* ix, void* stream, float* h_norm_max, float* h_max
 
 size_t rpx_index_topk_workspace_bytes(int64_t n, int32_t d, int32_t nq, int32_t k) {
   if (nq < 1 || k < 1 || k > 1024 || n < 0 || d <= 0) return 0;
-  const size_t a = ws_layout(n, nq, k, d, kMaxSmsForSizing).total, b = ws_layout(n, nq, k, d, 148).total;
+  const size_t a = ws_layout(n, nq, k, d, kMaxSmsForSizing).total, b = ws_layout(n, nq, k, d, 132).total;
   return (a > b ? a : b) + 256;
 }
 

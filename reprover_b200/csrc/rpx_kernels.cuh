@@ -12,7 +12,7 @@ namespace rpx {
 // bias_lut [heads][2*max_distance+1] fp32, entry (delta + max_distance), delta = key - query clamped.
 int launch_t5_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, const int32_t* cu_seqlens,
                         const float* bias_lut, int n_tokens, int n_seqs, int max_len, int n_heads, int d_kv,
-                        int max_distance, cudaStream_t stream, bool latency = false);
+                        int max_distance, cudaStream_t stream);
 
 // ---- rpx_elementwise.cu
 // ByT5 tokenisation of packed byte strings into packed token ids (byte + 3, EOS = 1 last,
@@ -39,7 +39,7 @@ int launch_pool_normalize(const float* h32, const float* ss, int ss_stride, int 
 int launch_pack_weight(const float* src, const float* scale, __nv_bfloat16* dst, int n_rows, int n_cols,
                        int dst_row0, int blk, int blk_stride, cudaStream_t stream);
 
-// ---- top-k paths (rpx_simtopk.cu: tcgen05, rpx_smallq.cu: HBM streaming, rpx_exact.cu: exact fp64)
+// ---- top-k paths (rpx_simtopk.cu: wgmma, rpx_smallq.cu: HBM streaming, rpx_exact.cu: exact fp64)
 struct IndexState;
 struct ExactBound;
 // One similarity + top-k request (all pointers are device pointers).

@@ -4,9 +4,9 @@
 //     argsort(descending) ... first k accessible    (:308-322)
 //
 // Stage 1  sim_topk (gemm_tc_kernel<..., EpiSimTopk, M_FASTEST>):
-//   tcgen05 MMA of a 128-query block against 256-premise tiles streamed once from HBM
+//   wgmma of a 128-query block against 128-premise tiles streamed once from HBM
 //   by TMA; the [Q, N] score matrix is never written.  Each epilogue thread owns one
-//   query row in TMEM, compares its 256 scores against that query's running threshold
+//   query row of the accumulator tile, compares its 128 scores against that query's running threshold
 //   and appends the few survivors (score, index) to a per-(CTA, query) candidate list.
 //   When a list fills up, the warp compacts it: a warp-shuffle bisection finds a
 //   threshold that keeps ~KEEP best entries, and the threshold rises.
@@ -26,17 +26,14 @@ namespace rpx {
 
 namespace {
 
-constexpr int kSimBlockN = 256;
+constexpr int kSimBlockN = 128;
 #ifndef RPX_SIM_SAMPLE_TILES
-#define RPX_SIM_SAMPLE_TILES 32
+#define RPX_SIM_SAMPLE_TILES 64
 #endif
 #ifndef RPX_SIM_SEL_SLACK
 #define RPX_SIM_SEL_SLACK 16
 #endif
-constexpr int kSampleTiles = RPX_SIM_SAMPLE_TILES;  // 32 x 256 = 8192 sampled premises
-#ifndef RPX_SIM_2CTA
-#define RPX_SIM_2CTA 1  // 0: stage 1 always on the 1-CTA kernel
-#endif
+constexpr int kSampleTiles = RPX_SIM_SAMPLE_TILES;  // 64 x 128 = 8192 sampled premises
 constexpr int kSelSlack = RPX_SIM_SEL_SLACK;        // stage 2 re-scores between n_res and n_res + kSelSlack rows
 constexpr unsigned kFull = kFullMask;
 
@@ -61,10 +58,7 @@ struct SimTopkParams {
   int tiles_m;
 };
 
-// PAIRED: the epilogue runs inside the 2-CTA (cta_group::2) kernel.  CTA `rank` of pair p serves query
-// block 2*(p % (tiles_m/2)) + rank and corpus segment p / (tiles_m/2); lists, counters and stage 2 keep
-// the 1-CTA numbering  cta = query_block + segment * tiles_m.
-template <int EPL, int KEEP_, bool PAIRED = false>
+template <int EPL, int KEEP_>
 struct EpiSimTopk {
   static constexpr int CAP = 32 * EPL;
   static constexpr int KEEP = KEEP_;
@@ -72,7 +66,7 @@ struct EpiSimTopk {
   static_assert(KEEP + SLACK + 32 <= CAP, "list too small");
   using Params = SimTopkParams;
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = 4;  // one warp per TMEM lane group: a query's list has one writer
+  static constexpr int kWarps = 4;  // one warp per lane group: a query's list has one writer
 
   Params p;
   float thr;        // pass rule: score > thr
@@ -86,11 +80,7 @@ struct EpiSimTopk {
 
   __device__ EpiSimTopk(const Params& p_, uint8_t*, int row, int) : p(p_) {
     lane = row & 31;
-    int cta = blockIdx.x;
-    if (PAIRED) {
-      const int pair = blockIdx.x >> 1, half = p.tiles_m >> 1;
-      cta = 2 * (pair % half) + (int)cluster_ctarank() + (pair / half) * p.tiles_m;
-    }
+    const int cta = blockIdx.x;
     q = (cta % p.tiles_m) * kBlockM + row;
     active = q < p.nq;
     thr = -INFINITY;
@@ -277,8 +267,7 @@ struct EpiSimTopk {
       // all 32 fill together) that is typically a single lane, so the other warps are not held up
       if (__any_sync(kFull, count() > CAP - 32)) compact_warp(CAP - 64);
       uint32_t v[32];
-      tmem_ld_32x32(t.tmem + c, v);
-      tmem_ld_wait();
+      acc_ld32(t.acc + c, v);
       const int base = t.n0 + c;
       uint32_t word = 0xFFFFFFFFu;
       if (p.mask != nullptr && active) word = p.mask[(size_t)q * p.mask_stride + (base >> 5)];
@@ -330,8 +319,7 @@ struct EpiSampleScores {
     for (int c = 0; c < kSimBlockN; c += 32) {
       uint32_t v[32];
       if (c < t.n_cols) {
-        tmem_ld_32x32(t.tmem + c, v);
-        tmem_ld_wait();
+        acc_ld32(t.acc + c, v);
       }
       const int base = t.n0 + c;
       uint32_t word = 0u;
@@ -359,8 +347,8 @@ struct EpiSampleScores {
 // One CTA per query: gthr[q] = T - 1 for a key value T with count(sample key >= T) >= n_res (any such T is
 // a valid starting bound: that many premises reach it), or 0 when fewer than n_res sampled premises are
 // admissible.  T comes from a 1024-bin histogram of the keys between the smallest and the largest valid
-// sample key: one pass over the scores, one pass over shared memory, one block scan (the bisection this
-// replaces took 12 block-wide probes: 39 us per 1024 queries against ~5 us).  T is the lower edge of the
+// sample key: one pass over the scores, one pass over shared memory, one block scan (instead of the
+// dozen block-wide probes of a bisection).  T is the lower edge of the
 // bin in which the n_res-th best key falls, so stage 1 admits at most that bin's extra keys.
 // The kernel also resets the per-query bookkeeping stage 1 starts from (list counts, final thresholds, the
 // shared gmin / gcnt bound) — three memset launches less per call.
@@ -456,10 +444,9 @@ sample_threshold_kernel(const float* __restrict__ S, int ld, int n_cols, int n_r
 
 // ------------------------------------------------------------------------------------ stage 2
 
-// Threads per query in stage 2: 512 when few queries are in flight (one query's latency is what
-// matters: Q = 1 0.192 vs 0.202 ms, Q = 64 0.166 vs 0.178 ms), 256 when there are enough queries to
-// fill the GPU (4 CTAs per SM instead of 2 overlap the staging / bisection / gather phases of different
-// queries: Q = 1024 0.607 vs 0.627 ms).
+// Threads per query in stage 2: many when few queries are in flight (one query's latency is what
+// matters), 256 when there are enough queries to fill the GPU (more CTAs per SM overlap the staging /
+// selection / gather phases of different queries).
 constexpr int kSelThreadsLatency = 1024, kSelThreadsThroughput = 256, kSelThroughputMinQueries = 512;
 constexpr int kSelMax = 288;  // >= largest re-score set (k + margin + selection slack)
 
@@ -791,7 +778,6 @@ struct SimPlan {
   int epl, cap, keep, list_max, n_res;
   size_t sel_smem;
   int tiles_m, grid;
-  bool paired;  // stage 1 on the 2-CTA kernel: tiles_m is even, grid = 2 * pairs
   size_t cand_bytes, cnt_bytes, gthr_bytes, sample_bytes, total;
   int sample_tiles;  // corpus tiles scored by the sampling pass (0 = no sampling pass)
 };
@@ -814,11 +800,7 @@ int plan_sim(int nq, int k, int d, int num_sms, SimPlan* pl) {
   pl->cap = 32 * pl->epl;
   int chunk_q = nq < num_sms * kBlockM ? nq : num_sms * kBlockM;  // queries per launch
   pl->tiles_m = ceil_div(chunk_q, kBlockM);
-  // two or more query blocks: stage 1 runs on CTA pairs (256 queries x 256 premises per tcgen05
-  // instruction); an odd block count is padded with an inactive block
-  pl->paired = RPX_SIM_2CTA && pl->tiles_m >= 2;
-  if (pl->paired) pl->tiles_m += pl->tiles_m & 1;
-  int n_seg = pl->paired ? (num_sms / 2) / (pl->tiles_m / 2) : num_sms / pl->tiles_m;
+  int n_seg = num_sms / pl->tiles_m;
   if (n_seg < 1) n_seg = 1;
   // stage 2 keeps one query's lists in shared memory: full-length lists if they fit, else lists
   // compacted to KEEP+16 at the end of stage 1, else fewer stage-1 CTAs per query block
@@ -831,7 +813,7 @@ int plan_sim(int nq, int k, int d, int num_sms, SimPlan* pl) {
   pl->cand_bytes = align_up((size_t)pl->grid * kBlockM * pl->cap * sizeof(uint2), 256);
   pl->cnt_bytes = align_up((size_t)pl->grid * kBlockM * sizeof(int32_t), 256);  // also the size of thr_out
   pl->gthr_bytes = align_up((size_t)pl->tiles_m * kBlockM * sizeof(uint32_t), 256);
-  // sampling pass: up to kSampleTiles tiles of 256 premises, score matrix capped at 64 MB
+  // sampling pass: up to kSampleTiles tiles of kSimBlockN premises, score matrix capped at 64 MB
   pl->sample_tiles = kSampleTiles;
   while (pl->sample_tiles > 4 &&
          (size_t)pl->tiles_m * kBlockM * pl->sample_tiles * kSimBlockN * sizeof(float) > (size_t)64 << 20)
@@ -870,34 +852,6 @@ int launch_sim_epi(const __nv_bfloat16* Q, int nq, const __nv_bfloat16* E, int64
   return RPX_OK;
 }
 
-// Stage 1 on the 2-CTA kernel (plan.paired): pairs = (tiles_m / 2) x segments.
-template <class Epi>
-int launch_sim_epi_paired(const __nv_bfloat16* Q, int nq, const __nv_bfloat16* E, int64_t n, int d,
-                          const typename Epi::Params& ep, const SimPlan& pl, cudaStream_t st) {
-  using Cfg = Gemm2Cfg<kGemm2Stages>;
-  DeviceInfo dev;
-  RPX_TRY(get_device_info(&dev));
-  CUtensorMap tmA, tmB;
-  RPX_TRY(make_tmap_bf16_2d(&tmA, Q, (uint64_t)nq, (uint64_t)d, (uint64_t)d, kBlockM));
-  RPX_TRY(make_tmap_bf16_2d(&tmB, E, (uint64_t)n, (uint64_t)d, (uint64_t)d, Cfg::kBlockN / 2));
-  const int tiles_m2 = pl.tiles_m / 2;
-  const int tiles_n = (int)ceil_div64(n, kSimBlockN);
-  const size_t smem = Cfg::smem_bytes(Epi::kSmemBytes);
-  RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "sim: needs %zu B smem, device allows %zu", smem,
-              dev.smem_optin);
-  auto kern = gemm_tc2_kernel<kGemm2Stages, Epi, true>;
-  static thread_local int configured_dev = -1;
-  if (configured_dev != dev.device) {
-    RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured_dev = dev.device;
-  }
-  const int64_t tiles = (int64_t)tiles_m2 * tiles_n;
-  const int pairs = tiles < pl.grid / 2 ? (int)tiles : pl.grid / 2;  // stays a multiple of tiles_m2
-  kern<<<2 * pairs, gemm_threads<Epi>(), smem, st>>>(tmA, tmB, pl.tiles_m * kBlockM, (int)n, d, tiles_m2, tiles_n, ep);
-  RPX_CUDA_OK(cudaGetLastError());
-  return RPX_OK;
-}
-
 }  // namespace
 
 size_t mma_topk_workspace_bytes(int nq, int k, int d, int num_sms) {
@@ -906,7 +860,7 @@ size_t mma_topk_workspace_bytes(int nq, int k, int d, int num_sms) {
   return pl.total + 256;
 }
 
-// The tcgen05 path: [stage 0 sampling pass + threshold] -> stage 1 (fused MMA + top-k epilogue) ->
+// The tensor-core path: [stage 0 sampling pass + threshold] -> stage 1 (fused MMA + top-k epilogue) ->
 // stage 2 (select, fp64 re-score, rank, guard).  `ws` is this path's private workspace.
 int run_mma_topk(const TopkCall& c, void* ws, size_t ws_bytes) {
   const int nq = c.nq, d = c.d, k = c.k;
@@ -965,13 +919,7 @@ int run_mma_topk(const TopkCall& c, void* ws, size_t ws_bytes) {
     }
     if (n > 0) {
       SimTopkParams ep{cand, cnt, thr_out, gthr, gmin, gcnt, n_seg, rank_r, pl.list_max, mask_c, c.mask_stride, nq_c, (int)n, pl.tiles_m};
-      if (pl.paired) {
-        if (pl.keep == 128) {
-          RPX_TRY((launch_sim_epi_paired<EpiSimTopk<16, 128, true>>(Q + (size_t)q0 * d, nq_c, E, n, d, ep, pl, st)));
-        } else {
-          RPX_TRY((launch_sim_epi_paired<EpiSimTopk<16, 256, true>>(Q + (size_t)q0 * d, nq_c, E, n, d, ep, pl, st)));
-        }
-      } else if (pl.keep == 128) {
+      if (pl.keep == 128) {
         RPX_TRY((launch_sim_epi<EpiSimTopk<16, 128>>(Q + (size_t)q0 * d, nq_c, E, n, d, ep, pl, st)));
       } else {
         RPX_TRY((launch_sim_epi<EpiSimTopk<16, 256>>(Q + (size_t)q0 * d, nq_c, E, n, d, ep, pl, st)));

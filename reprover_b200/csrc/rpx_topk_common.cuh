@@ -1,5 +1,5 @@
 // rpx_topk_common.cuh — device helpers shared by the three top-k paths
-// (rpx_simtopk.cu: tcgen05 path, rpx_smallq.cu: HBM-streaming path for <= 4 queries,
+// (rpx_simtopk.cu: tensor-core path, rpx_smallq.cu: HBM-streaming path for <= 4 queries,
 //  rpx_exact.cu: exact fp64 fallback) and the device-resident state of an index handle.
 //
 // Ordering contract (include/rpx.h): score descending, then index ascending, where score is the
@@ -153,7 +153,7 @@ __device__ __forceinline__ double dot64_canonical(const __nv_bfloat16* __restric
 // A fast path ranks rows by an fp32 score s32 that differs from the contract's fp64 score s64 by at
 // most eps = c(d) * ||q||_2 * max_i ||e_i||_2  (|sum of products| and every partial sum are bounded
 // by sum |q_j e_ij| <= ||q|| ||e_i||):
-//   tcgen05 path   every K=16 instruction adds 16 exact products to the fp32 accumulator; each addend
+//   wgmma path     every K=16 instruction adds 16 exact products to the fp32 accumulator; each addend
 //                  may lose < 1 ulp of the largest magnitude involved when it is aligned, and the
 //                  result is rounded once more: <= 18 * 2^-23 * sum|p| per instruction, d/16
 //                  instructions  ->  c = (18 d / 16 + 2) * 2^-23   (2.0e-4 for d = 1472)

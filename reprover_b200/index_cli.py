@@ -1,4 +1,4 @@
-"""Index a corpus with the B200 engine.  Same flags and output format as the reference's
+"""Index a corpus with the H100 engine.  Same flags and output format as the reference's
 `retrieval/index.py` (--ckpt_path, --corpus-path, --output-path, --batch-size; writes a pickled
 `IndexedCorpus` with fp32 CPU embeddings, retrieval/index.py:33-40), so the result can be
 handed to anything that calls `load_corpus(indexed_corpus_path)`.
@@ -22,7 +22,7 @@ logger = logging.getLogger("reprover_b200.index")
 
 
 def main(argv=None) -> None:
-    parser = argparse.ArgumentParser(description="Index a premise corpus with the B200 retrieval engine.")
+    parser = argparse.ArgumentParser(description="Index a premise corpus with the H100 retrieval engine.")
     parser.add_argument("--ckpt_path", type=str, required=True)
     parser.add_argument("--corpus-path", type=str, required=True)
     parser.add_argument("--output-path", type=str, required=True)
@@ -35,7 +35,7 @@ def main(argv=None) -> None:
     logger.info(args)
     if not torch.cuda.is_available():
         # the reference falls back to the CPU with a warning (index.py:28-30); this engine does not
-        raise SystemExit("reprover_b200 needs a B200 GPU: there is no CPU indexing path")
+        raise SystemExit("reprover_b200 needs an H100 GPU: there is no CPU indexing path")
     import os
 
     world = int(os.environ.get("WORLD_SIZE", "1"))

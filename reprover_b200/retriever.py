@@ -58,7 +58,7 @@ class B200PremiseRetriever:
         self.max_seq_len = max_seq_len
         self.device = device
         # Reference dtype policy (retrieval/model.py:56-66): bf16 on GPUs with cc >= 8 unless told
-        # otherwise — on a B200 that is bf16, which is the one compute dtype this engine has (bf16
+        # otherwise — on an H100 that is bf16, which is the one compute dtype this engine has (bf16
         # operands, fp32 accumulation, fp32 residual stream; similarity index held in bf16 like the
         # reference's GPU path, :363-366).  `dtype=torch.float32` in the reference means an fp32 MODEL
         # and an fp32 index; quietly running bf16 under that name would misreport what was computed, so

@@ -1,4 +1,4 @@
-"""pytest configuration: registers the `gpu` marker (tests that need a real B200)."""
+"""pytest configuration: registers the `gpu` marker (tests that need a real H100)."""
 import os
 import sys
 from pathlib import Path
@@ -11,7 +11,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200, sm_100a); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a); run with -m gpu")
 
 
 @pytest.fixture(scope="session")
@@ -29,7 +29,7 @@ def cuda_device():
     import torch
 
     if not torch.cuda.is_available():
-        pytest.fail("a `gpu`-marked test ran without a CUDA device (select with -m gpu on a B200 box)")
+        pytest.fail("a `gpu`-marked test ran without a CUDA device (select with -m gpu on an H100 machine)")
     return torch.device("cuda:0")
 
 

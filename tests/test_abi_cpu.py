@@ -37,13 +37,13 @@ def test_library_has_no_libcuda_dependency():
     assert "libcuda.so" not in out
 
 
-def test_sass_is_blackwell_native():
-    """The cubin carries tcgen05 MMA / TMEM / TMA instructions (UTC*MMA, LDTM, UTMALDG), sm_100a only."""
+def test_sass_is_hopper_native():
+    """The cubin carries warpgroup MMA and TMA instructions (HGMMA, UTMALDG), sm_90a only."""
     import subprocess
 
     sass = subprocess.run(["cuobjdump", "-sass", str(_native.library_path())], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "LDTM", "UTMALDG"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA", "UTMALDG"):
         assert mnemonic in sass, mnemonic
 
 

@@ -236,8 +236,8 @@ def test_many_short_sequences_and_chunking(rpx_lib, cuda_device, tiny):
 
 def test_byt5_small_full_size_batch_invariance(rpx_lib, cuda_device):
     """BASELINE config 2 geometry at a size where every pipelined path is busy: 1500 premises = one
-    full 262,144-token engine call (74 CTA pairs x ~83 tiles each: operand ring, TMEM double buffer
-    and the residual TMA ring all run across many tile boundaries) plus a ragged tail call.  An
+    full 262,144-token engine call (many tiles per persistent CTA: the operand ring and the accumulator
+    hand-off run across many tile boundaries) plus a ragged tail call.  An
     embedding must not depend on what else is in the batch — bit for bit: every output row sums its
     products in an order fixed by the kernel shapes, not by the tile, the pair or the call it lands
     in — and the sampled rows must still match the fp32 oracle."""

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05/TMA/TMEM contraction core against a plain PyTorch fp32 matmul
+"""Parity of the wgmma/TMA contraction core against a plain PyTorch fp32 matmul
 of the same bf16 operands (C = A @ B^T, fp32 accumulate)."""
 import json
 
@@ -15,7 +15,7 @@ ENTRY = "rpx_gemm_bf16_f32"
 
 @pytest.fixture(params=["rpx_gemm_bf16_f32", "rpx_gemm2_bf16_f32"], autouse=True)
 def _entry(request):
-    """Every test runs through both the 1-CTA and the 2-CTA (cta_group::2) form of the core."""
+    """Every test runs through both the single-CTA and the paired (2-CTA cluster, multicast B) form of the core."""
     global ENTRY
     ENTRY = request.param
     yield
@@ -60,9 +60,9 @@ def _diagnose(C, R, tag, out_dir):
         (256, 512, 384),     # 2x2 tiles
         (300, 1472, 384),    # ragged M, ragged N tail (192 cols), o-proj shape
         (1000, 1152, 1472),  # qkv shape, N tail 128
-        (4096, 7168, 1472),  # ffn-up shape, many tiles per CTA (persistent loop + TMEM double buffer)
+        (4096, 7168, 1472),  # ffn-up shape, many tiles per CTA (persistent loop, accumulator tile hand-off)
         (777, 1472, 3584),   # ffn-down shape
-        (20000, 256, 128),   # >148 tiles along M
+        (20000, 256, 128),   # >132 tiles along M
     ],
 )
 def test_gemm_matches_torch(rpx_lib, cuda_device, out_dir, M, N, K):

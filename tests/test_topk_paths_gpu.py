@@ -1,4 +1,4 @@
-"""The three top-k paths behind `rpx_index_topk` — tcgen05 (any Q), HBM-streaming (Q <= 4) and
+"""The three top-k paths behind `rpx_index_topk` — tensor core (any Q), HBM-streaming (Q <= 4) and
 exact fp64 — each pinned through the C ABI against the C oracle (`oracle/rpx_oracle.c`): indices and
 fp64 scores bit-exact under (score desc, index asc).  Includes the inputs the fp32 fast paths cannot
 rank by themselves (near-ties far below fp32 accumulation noise): the exactness guard must hand those

@@ -1,4 +1,4 @@
-"""Quick device-side timing of the bare tcgen05 GEMM at the encoder's shapes (CUDA events)."""
+"""Quick device-side timing of the bare wgmma GEMM at the encoder's shapes, single-CTA and paired form (CUDA events)."""
 import json, sys
 from pathlib import Path
 import torch
@@ -13,17 +13,21 @@ for (M, N, K) in [(65536, 7168, 1472), (65536, 1472, 3584), (65536, 1152, 1472),
     B = torch.randn(N, K, device=dev).to(torch.bfloat16)
     C = torch.empty(M, N, device=dev)
     st = torch.cuda.current_stream().cuda_stream
-    for _ in range(3):
-        _native.check(lib.rpx_gemm_bf16_f32(A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, st))
-    torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     reps = 10
-    e0.record()
-    for _ in range(reps):
-        lib.rpx_gemm_bf16_f32(A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, st)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / reps
+    times = {}
+    for entry in ("rpx_gemm_bf16_f32", "rpx_gemm2_bf16_f32"):
+        fn = getattr(lib, entry)
+        for _ in range(3):
+            _native.check(fn(A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, st))
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(reps):
+            fn(A.data_ptr(), B.data_ptr(), C.data_ptr(), M, N, K, st)
+        e1.record()
+        torch.cuda.synchronize()
+        times[entry] = e0.elapsed_time(e1) / reps
+    ms, ms2 = times["rpx_gemm_bf16_f32"], times["rpx_gemm2_bf16_f32"]
     # cuBLAS reference point (library GEMM, not part of the product path)
     Cb = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
     for _ in range(3):
@@ -36,7 +40,8 @@ for (M, N, K) in [(65536, 7168, 1472), (65536, 1472, 3584), (65536, 1152, 1472),
     torch.cuda.synchronize()
     ms_b = e0.elapsed_time(e1) / reps
     tf = 2.0 * M * N * K / ms / 1e9
-    out[f"{M}x{N}x{K}"] = {"ms": ms, "tflops": tf, "cublas_ms": ms_b, "cublas_tflops": 2.0 * M * N * K / ms_b / 1e9}
-    print(M, N, K, f"{ms:.3f} ms  {tf:.1f} TF/s   cublas {ms_b:.3f} ms", flush=True)
+    out[f"{M}x{N}x{K}"] = {"ms": ms, "tflops": tf, "paired_ms": ms2, "cublas_ms": ms_b,
+                           "cublas_tflops": 2.0 * M * N * K / ms_b / 1e9}
+    print(M, N, K, f"{ms:.3f} ms  {tf:.1f} TF/s   paired {ms2:.3f} ms   cublas {ms_b:.3f} ms", flush=True)
 Path("gpurun_out").mkdir(exist_ok=True)
 Path("gpurun_out/gemm_bench.json").write_text(json.dumps(out, indent=1))
