@@ -27,8 +27,10 @@ namespace rpx {
 
 namespace {
 
-// Throughput-path tiles: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand ring fit the 227 KB of
-// shared memory an H100 block may use; the gated FFN up-projection runs them as split-B tiles of 64 hidden units.
+// Throughput-path tiles of QKV, O-proj and FFN-down: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand
+// ring fit the 227 KB of shared memory an H100 block may use.  The gated FFN up-projection runs on gemm_ws_kernel's
+// 128 x 256 tiles instead (rpx_gemm_ws.cuh): on an H100 it measured 12 % faster there, while the other three
+// GEMMs measured 6-18 % slower, their epilogues no longer overlapping the next tile's MMAs.
 constexpr int kBlockN = 128;
 
 // h32 += A @ B^T, h16 = bf16(h32), ss = partial sums of h32^2 per n-tile.
@@ -221,7 +223,7 @@ struct Prof {
 
 // ---------------------------------------------------------------------------------------------
 // Latency path: one proof state per call (`retrieve`, retrieval/model.py:348-357, encodes ONE context).
-// With T of a few hundred tokens the 128 x 128 tiles of the throughput path leave most of the GPU idle
+// With T of a few hundred tokens the 128-row tiles of the throughput path leave most of the GPU idle
 // (QKV: 9 tiles, O / FFN-down: 12 tiles for a 128-token state) and every GEMM is bound by the latency of
 // streaming its operands through a handful of SMs.  Here the same contraction core runs narrow tiles:
 //   up to 384 tokens   QKV, O-proj, FFN-down on 64-ROW tiles (one wgmma row block) x 64 columns with a 12-deep
@@ -351,8 +353,8 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     }
     {
       Prof p(e, st, 4);
-      EpiGeGLUT<kBlockN / 2>::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((launch_gemm<kBlockN, EpiGeGLUT<kBlockN / 2>, false, kGemmStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
+      EpiWsGeGLU::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
+      RPX_TRY(launch_gemm_ws<EpiWsGeGLU>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st));
     }
     {
       Prof p(e, st, 5);

@@ -614,9 +614,9 @@ __device__ __forceinline__ float gelu_new(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
-// Gated-GELU FFN up projection (K9): accumulator columns [0, HALF) are the gate and [HALF, 2*HALF) the
-// linear branch of the same HALF hidden units (HALF = 128: the 256-wide tiles of the throughput path, whose B
-// operand interleaves wi_0 / wi_1 in 128-row blocks; HALF = 64 / 32: the SPLIT_B narrow tiles).
+// Gated-GELU FFN up projection (K9) of the latency path: accumulator columns [0, HALF) are the gate and
+// [HALF, 2*HALF) the linear branch of the same HALF hidden units (HALF = 64 / 32: the SPLIT_B tiles).  The
+// throughput path runs EpiWsGeGLU (rpx_gemm_ws.cuh).
 //   out[m, n_blk*HALF + j] = bf16( gelu_new(acc[j]*rs) * (acc[HALF+j]*rs) )
 template <int HALF>
 struct EpiGeGLUT {
@@ -661,6 +661,5 @@ struct EpiGeGLUT {
   }
   __device__ void finish() {}
 };
-using EpiGeGLU = EpiGeGLUT<128>;
 
 }  // namespace rpx

@@ -1,7 +1,8 @@
-// rpx_gemm_launch.cuh — host-side launcher for gemm_tc_kernel.
+// rpx_gemm_launch.cuh — host-side launchers for gemm_tc_kernel and gemm_ws_kernel.
 #pragma once
 #include "rpx_common.cuh"
 #include "rpx_gemm.cuh"
+#include "rpx_gemm_ws.cuh"
 
 namespace rpx {
 
@@ -45,6 +46,37 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
     grid = dev.num_sms;  // surplus SMs run prefetch helpers
   RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(gemm_threads<Epi>()), smem, stream, pdl_enabled(), tmA, tmB, M, N, K, tiles_m,
                          tiles_n, 1, ep, pf));
+  return RPX_OK;
+}
+
+// Throughput core (gemm_ws_kernel): 128 x 256 tiles, persistent over one CTA per SM.
+// A: [M, K] bf16 (row pitch lda), B: [N, K] bf16 (row pitch ldb).  K % 64 == 0, N % 32 == 0.
+template <class Epi>
+int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
+                   const typename Epi::Params& ep, cudaStream_t stream) {
+  RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
+  RPX_REQUIRE(K % kBlockK == 0, RPX_ERR_UNSUPPORTED, "gemm: K=%d must be a multiple of %d", K, kBlockK);
+  RPX_REQUIRE(N % 32 == 0, RPX_ERR_UNSUPPORTED, "gemm: N=%d must be a multiple of 32", N);
+  DeviceInfo dev;
+  RPX_TRY(get_device_info(&dev));
+  CUtensorMap tmA, tmB;
+  RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, kBlockM));
+  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, kWsBlockN));
+  const int tiles_m = ceil_div(M, kBlockM);
+  const int tiles_n = ceil_div(N, kWsBlockN);
+  const size_t smem = WsCfg::kSmemBytes;
+  RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu", smem,
+              dev.smem_optin);
+  auto kern = gemm_ws_kernel<Epi>;
+  static thread_local int configured_dev = -1;  // per-instantiation, per-thread
+  if (configured_dev != dev.device) {
+    RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured_dev = dev.device;
+  }
+  int grid = tiles_m * tiles_n;
+  if (grid > dev.num_sms) grid = dev.num_sms;
+  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA, tmB, M, N, K, tiles_m,
+                         tiles_n, ep));
   return RPX_OK;
 }
 

@@ -1,4 +1,4 @@
-"""Quick device-side timing of the bare wgmma GEMM at the encoder's shapes, single-CTA and paired form (CUDA events)."""
+"""Device-side timing (CUDA events) of the bare GEMM cores at the encoder's shapes for one 2^18-token call: rpx_gemm_bf16_f32 (128 x 256 throughput core), rpx_gemm2_bf16_f32 (paired 128 x 128 form) and cuBLAS."""
 import json, sys
 from pathlib import Path
 import torch
@@ -8,7 +8,7 @@ from reprover_b200 import _native
 lib = _native.load()
 dev = torch.device("cuda:0")
 out = {}
-for (M, N, K) in [(65536, 7168, 1472), (65536, 1472, 3584), (65536, 1152, 1472), (65536, 1472, 384), (16384, 7168, 1472)]:
+for (M, N, K) in [(262144, 7168, 1472), (262144, 1472, 3584), (262144, 1152, 1472), (262144, 1472, 384)]:
     A = torch.randn(M, K, device=dev).to(torch.bfloat16)
     B = torch.randn(N, K, device=dev).to(torch.bfloat16)
     C = torch.empty(M, N, device=dev)
