@@ -246,10 +246,28 @@ int rpx_debug_set_timeline(unsigned long long* d_stamps, int32_t n_slots);
  * C[M, N] (fp32, ldc = N) = A[M, K] * B[N, K]^T, bf16 inputs; K % 64 == 0, N % 32 == 0. */
 int rpx_gemm_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                       int32_t K, void* stream);
+/* Same contract through the single-CTA 128 x 128 core that runs QKV, O-proj and FFN-down on the
+ * throughput path and every GEMM of the latency path. */
+int rpx_gemm1_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
+                       int32_t K, void* stream);
 /* Same contract through the paired form of the core: clusters of two CTAs on vertically adjacent
  * 128 x 128 tiles that share each B tile through TMA multicast. */
 int rpx_gemm2_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                        int32_t K, void* stream);
+
+enum { RPX_EGEMM_QKV = 0, RPX_EGEMM_OPROJ = 1, RPX_EGEMM_FFN_UP = 2, RPX_EGEMM_FFN_DOWN = 3 };
+/* One encoder GEMM, launched as the forward pass launches it for T tokens on the throughput (latency = 0) or
+ * latency path, PDL scope set as forward() sets it for that T.  A [T, K] bf16 (lda = K), B [N, K] bf16 in the
+ * packed layout rpx_encoder_create writes.  D = d_model = K for QKV / FFN-up, N for O-proj / FFN-down.
+ *   QKV     out [T, N] bf16 = bf16(A B^T * rs[m]),  rs from ss_in
+ *   FFN_UP  out [T, N/2] bf16 gated GELU,             rs from ss_in;  N % 256 == 0
+ *   OPROJ / FFN_DOWN   h32 [T, N] += A B^T;  h16 = bf16(h32);  ss_out partials
+ * ss_in / ss_out: [parts][T] fp32, parts = ceil(D / 128) (throughput) or D / 32 (latency).
+ * d_prefetch (latency QKV only, else NULL): prefetch_bytes fetched into L2 by the CTAs the GEMM leaves idle. */
+int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const void* d_B, int32_t T,
+                           int32_t N, int32_t K, float ln_eps, const float* d_ss_in, void* d_out,
+                           float* d_h32, void* d_h16, float* d_ss_out, const void* d_prefetch,
+                           size_t prefetch_bytes, void* stream);
 
 #ifdef __cplusplus
 }

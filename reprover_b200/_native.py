@@ -111,9 +111,19 @@ _SIGNATURES = {
     "rpx_debug_set_timeline": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_gemm_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p]),
+    "rpx_gemm1_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_void_p]),
     "rpx_gemm2_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_void_p]),
+    "rpx_debug_encoder_gemm": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                         C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
+
+RPX_EGEMM_QKV = 0
+RPX_EGEMM_OPROJ = 1
+RPX_EGEMM_FFN_UP = 2
+RPX_EGEMM_FFN_DOWN = 3
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

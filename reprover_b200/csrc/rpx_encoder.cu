@@ -33,13 +33,6 @@ namespace {
 // GEMMs measured 6-18 % slower, their epilogues no longer overlapping the next tile's MMAs.
 constexpr int kBlockN = 128;
 
-// h32 += A @ B^T, h16 = bf16(h32), ss = partial sums of h32^2 per n-tile.
-int residual_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int T, int D, int K, float* h32,
-                  __nv_bfloat16* h16, float* ss, cudaStream_t st) {
-  EpiResidual::Params ep{h32, h16, D, ss, T};
-  return launch_gemm<kBlockN, EpiResidual>(A, lda, B, ldb, T, D, K, ep, st);
-}
-
 struct LayerW {
   const __nv_bfloat16* qkv;  // [3*inner, D]   (ln0 folded)
   const __nv_bfloat16* o;    // [D, inner]
@@ -246,6 +239,70 @@ constexpr int kLatSmallMMaxTokens = 384;
 // noticeable share of a kernel's time.
 constexpr int kPdlMaxTokens = 16384;
 
+struct PdlScope {
+  explicit PdlScope(bool on) { set_pdl_scope(on); }
+  ~PdlScope() { set_pdl_scope(false); }
+};
+
+// RMSNorm partial sums per row: one per 128-wide n-tile on the throughput path, one per 32-column chunk on the
+// latency path.
+int ss_parts(int d_model, bool latency) {
+  return ceil_div(d_model, latency ? 32 : kBlockN) * (EpiResidual::kWarps / 4);
+}
+
+// The encoder's four GEMMs, each on the tiles the forward pass uses for T tokens on the throughput or the
+// latency path.  forward(), forward_latency_layer() and rpx_debug_encoder_gemm all launch through these, so the
+// epilogue tests run exactly the launches an encode call runs.  A is [T, K], B is [N, K] (packed weights).
+
+// out [T, N] = bf16(A B^T * rs[m]).  On the latency path the CTAs the GEMM leaves idle fetch `prefetch` into L2.
+int qkv_gemm(bool latency, int T, const void* A, const void* B, int N, int K, const RowScale& rs, __nv_bfloat16* out,
+             const void* prefetch, size_t prefetch_bytes, cudaStream_t st) {
+  EpiStoreBF16::Params ep{out, N, rs};
+  if (!latency) return launch_gemm<kBlockN, EpiStoreBF16>(A, K, B, K, T, N, K, ep, st);
+  if (T <= kLatSmallMMaxTokens)
+    return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st, 0,
+                                                                                             prefetch, prefetch_bytes);
+  return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatStages>(A, K, B, K, T, N, K, ep, st, 0, prefetch, prefetch_bytes);
+}
+
+// h32 [T, N] += A B^T, h16 = bf16(h32), ss_out = partial sums of h32^2 ([ss_parts(N)][T]).
+int residual_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
+                  float* ss_out, cudaStream_t st) {
+  EpiResidualParams ep{h32, h16, N, ss_out, T};
+  if (!latency) return launch_gemm<kBlockN, EpiResidual>(A, K, B, K, T, N, K, ep, st);
+  if (T <= kLatSmallMMaxTokens)
+    return launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st);
+  return launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatStages>(A, K, B, K, T, N, K, ep, st);
+}
+int oproj_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
+               float* ss_out, cudaStream_t st) {
+  return residual_gemm(latency, T, A, B, N, K, h32, h16, ss_out, st);
+}
+int ffn_down_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
+                  float* ss_out, cudaStream_t st) {
+  return residual_gemm(latency, T, A, B, N, K, h32, h16, ss_out, st);
+}
+
+// out [T, N/2] = bf16(gelu_new(A B^T_gate * rs[m]) * (A B^T_linear * rs[m])).  B interleaves the gate and linear
+// rows in 128-row blocks (rpx_encoder_create), and every tile pairs gate column j with linear column j + 128 of
+// its 256-row block, so N must be a whole number of such blocks.
+int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K, const RowScale& rs,
+                __nv_bfloat16* out, cudaStream_t st) {
+  RPX_REQUIRE(N % 256 == 0, RPX_ERR_UNSUPPORTED, "ffn-up gemm: N=%d must be a multiple of 256 (2 x d_ff, d_ff %% 128 == 0)", N);
+  const int F = N / 2;
+  if (!latency) {
+    EpiWsGeGLU::Params ep{out, F, rs};
+    return launch_gemm_ws<EpiWsGeGLU>(A, K, B, K, T, N, K, ep, st);
+  }
+  // hidden units per tile: 32 (64-column tiles, T <= 128: 112 CTAs) or 64 (128-column tiles: 56 x ceil(T/128))
+  if (T <= kBlockM) {
+    EpiGeGLUT<32>::Params ep{out, F, rs};
+    return launch_gemm<64, EpiGeGLUT<32>, false, kLatStages, true>(A, K, B, K, T, N, K, ep, st);
+  }
+  EpiGeGLUT<64>::Params ep{out, F, rs};
+  return launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(A, K, B, K, T, N, K, ep, st);
+}
+
 int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, const void* next_weights,
                           size_t next_bytes, int T, int S, int max_len, cudaStream_t st) {
   const rpx_t5_config& c = e->cfg;
@@ -253,17 +310,10 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   const float inv_d = 1.0f / (float)D;
   {
     Prof p(e, st, 1);
-    EpiStoreBF16::Params ep{ws.qkv, 3 * inner, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}};
     // the QKV projection occupies 18 x ceil(T/64) (or 18 x ceil(T/128)) SMs for 6 heads: the rest of the GPU
     // fetches the next layer's weights into L2
-    if (T <= kLatSmallMMaxTokens) {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(ws.h16, D, w.qkv, D, T, 3 * inner,
-                                                                                                 D, ep, st, 0, next_weights,
-                                                                                                 next_bytes)));
-    } else {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatStages>(ws.h16, D, w.qkv, D, T, 3 * inner, D, ep, st, 0,
-                                                                         next_weights, next_bytes)));
-    }
+    RPX_TRY(qkv_gemm(true, T, ws.h16, w.qkv, 3 * inner, D, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}, ws.qkv, next_weights,
+                     next_bytes, st));
   }
   {
     Prof p(e, st, 2);
@@ -272,34 +322,15 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   }
   {
     Prof p(e, st, 3);
-    EpiResidual::Params ep{ws.h32, ws.h16, D, ws.ssB, T};
-    if (T <= kLatSmallMMaxTokens) {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatSmallStages, false, kLatSmallM>(ws.attn, inner, w.o, inner, T,
-                                                                                                       D, inner, ep, st)));
-    } else {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatStages>(ws.attn, inner, w.o, inner, T, D, inner, ep, st)));
-    }
+    RPX_TRY(oproj_gemm(true, T, ws.attn, w.o, D, inner, ws.h32, ws.h16, ws.ssB, st));
   }
   {
     Prof p(e, st, 4);
-    // hidden units per tile: 32 (64-column tiles, T <= 128: 112 CTAs) or 64 (128-column tiles: 56 x ceil(T/128))
-    if (T <= kBlockM) {
-      EpiGeGLUT<32>::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((launch_gemm<64, EpiGeGLUT<32>, false, kLatStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
-    } else {
-      EpiGeGLUT<64>::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st)));
-    }
+    RPX_TRY(ffn_up_gemm(true, T, ws.h16, w.wi, 2 * F, D, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}, ws.ffn, st));
   }
   {
     Prof p(e, st, 5);
-    EpiResidual::Params ep{ws.h32, ws.h16, D, ws.ssA, T};
-    if (T <= kLatSmallMMaxTokens) {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatSmallStages, false, kLatSmallM>(ws.ffn, F, w.wo, F, T, D, F,
-                                                                                                       ep, st)));
-    } else {
-      RPX_TRY((launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatStages>(ws.ffn, F, w.wo, F, T, D, F, ep, st)));
-    }
+    RPX_TRY(ffn_down_gemm(true, T, ws.ffn, w.wo, D, F, ws.h32, ws.h16, ws.ssA, st));
   }
   return RPX_OK;
 }
@@ -313,10 +344,7 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
   const bool latency = T <= e->latency_tokens && D % 32 == 0 && (3 * inner) % 32 == 0;
   const int P = latency ? e->n_parts_lat : e->n_parts;
   const float inv_d = 1.0f / (float)D;
-  struct PdlScope {
-    explicit PdlScope(bool on) { set_pdl_scope(on); }
-    ~PdlScope() { set_pdl_scope(false); }
-  } pdl_scope(latency || T <= kPdlMaxTokens);
+  PdlScope pdl_scope(latency || T <= kPdlMaxTokens);
   {
     Prof p(e, st, 0);
     RPX_TRY(launch_embed(ws.ids, e->emb, ws.h32, ws.h16, ws.ssA, T, P, T, D, st));
@@ -339,8 +367,8 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     }
     {
       Prof p(e, st, 1);
-      EpiStoreBF16::Params ep{ws.qkv, 3 * inner, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}};
-      RPX_TRY((launch_gemm<kBlockN, EpiStoreBF16>(ws.h16, D, w.qkv, D, T, 3 * inner, D, ep, st)));
+      RPX_TRY(qkv_gemm(false, T, ws.h16, w.qkv, 3 * inner, D, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}, ws.qkv, nullptr, 0,
+                       st));
     }
     {
       Prof p(e, st, 2);
@@ -349,16 +377,15 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     }
     {
       Prof p(e, st, 3);
-      RPX_TRY(residual_gemm(ws.attn, inner, w.o, inner, T, D, inner, ws.h32, ws.h16, ws.ssB, st));
+      RPX_TRY(oproj_gemm(false, T, ws.attn, w.o, D, inner, ws.h32, ws.h16, ws.ssB, st));
     }
     {
       Prof p(e, st, 4);
-      EpiWsGeGLU::Params ep{ws.ffn, F, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}};
-      RPX_TRY(launch_gemm_ws<EpiWsGeGLU>(ws.h16, D, w.wi, D, T, 2 * F, D, ep, st));
+      RPX_TRY(ffn_up_gemm(false, T, ws.h16, w.wi, 2 * F, D, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}, ws.ffn, st));
     }
     {
       Prof p(e, st, 5);
-      RPX_TRY(residual_gemm(ws.ffn, F, w.wo, F, T, D, F, ws.h32, ws.h16, ws.ssA, st));
+      RPX_TRY(ffn_down_gemm(false, T, ws.ffn, w.wo, D, F, ws.h32, ws.h16, ws.ssA, st));
     }
     RPX_TRY(dump(l + 1));
   }
@@ -402,8 +429,8 @@ int rpx_encoder_create(const rpx_t5_config* cfg, const rpx_t5_weights* w, void* 
   RPX_REQUIRE(e != nullptr, RPX_ERR_INVALID, "out of host memory");
   e->cfg = *cfg;
   e->inner = inner;
-  e->n_parts = ceil_div(D, kBlockN) * (EpiResidual::kWarps / 4);
-  e->n_parts_lat = ceil_div(D, 32) * (EpiResidual::kWarps / 4);  // one per 32-column chunk
+  e->n_parts = ss_parts(D, false);
+  e->n_parts_lat = ss_parts(D, true);
   auto fail = [&](int code) {
     delete e;
     return code;
@@ -577,6 +604,35 @@ int rpx_encoder_set_profiling(rpx_encoder* enc, int32_t enable) {
   RPX_REQUIRE(enc, RPX_ERR_INVALID, "null encoder");
   enc->profiling = enable != 0;
   return RPX_OK;
+}
+
+int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const void* d_B, int32_t T, int32_t N,
+                           int32_t K, float ln_eps, const float* d_ss_in, void* d_out, float* d_h32, void* d_h16,
+                           float* d_ss_out, const void* d_prefetch, size_t prefetch_bytes, void* stream) {
+  RPX_REQUIRE(site >= RPX_EGEMM_QKV && site <= RPX_EGEMM_FFN_DOWN, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: site=%d", site);
+  RPX_REQUIRE(d_A && d_B, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: null operand");
+  RPX_REQUIRE(T > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: T=%d N=%d K=%d", T, N, K);
+  const bool lat = latency != 0;
+  const bool residual = site == RPX_EGEMM_OPROJ || site == RPX_EGEMM_FFN_DOWN;
+  const int D = residual ? N : K;
+  RPX_REQUIRE(D % 64 == 0, RPX_ERR_UNSUPPORTED, "rpx_debug_encoder_gemm: d_model=%d must be a multiple of 64", D);
+  if (residual)
+    RPX_REQUIRE(d_h32 && d_h16 && d_ss_out, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: residual site needs h32, h16, ss_out");
+  else
+    RPX_REQUIRE(d_ss_in && d_out, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: site %d needs ss_in and out", site);
+  RPX_REQUIRE(d_prefetch == nullptr || (lat && site == RPX_EGEMM_QKV), RPX_ERR_INVALID,
+              "rpx_debug_encoder_gemm: only the latency QKV projection prefetches");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PdlScope pdl_scope(lat || T <= kPdlMaxTokens);
+  const RowScale rs{d_ss_in, ss_parts(D, lat), T, 1.0f / (float)D, ln_eps};
+  auto* out = static_cast<__nv_bfloat16*>(d_out);
+  auto* h16 = static_cast<__nv_bfloat16*>(d_h16);
+  switch (site) {
+    case RPX_EGEMM_QKV: return qkv_gemm(lat, T, d_A, d_B, N, K, rs, out, d_prefetch, prefetch_bytes, st);
+    case RPX_EGEMM_OPROJ: return oproj_gemm(lat, T, d_A, d_B, N, K, d_h32, h16, d_ss_out, st);
+    case RPX_EGEMM_FFN_UP: return ffn_up_gemm(lat, T, d_A, d_B, N, K, rs, out, st);
+    default: return ffn_down_gemm(lat, T, d_A, d_B, N, K, d_h32, h16, d_ss_out, st);
+  }
 }
 
 int rpx_encoder_read_profile(rpx_encoder* enc, float* h_ms, int64_t* h_launches) {

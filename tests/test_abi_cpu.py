@@ -78,6 +78,14 @@ def test_compute_fails_loudly_without_gpu(rpx_lib):
     buf = (C.c_uint8 * 1024)()
     rc = rpx_lib.rpx_gemm_bf16_f32(buf, buf, buf, 128, 256, 64, None)
     assert rc == _native.RPX_ERR_CUDA and _native.last_error()
+    rc = rpx_lib.rpx_gemm1_bf16_f32(buf, buf, buf, 128, 256, 64, None)
+    assert rc == _native.RPX_ERR_CUDA and _native.last_error()
+    for site in (_native.RPX_EGEMM_QKV, _native.RPX_EGEMM_FFN_UP):
+        rc = rpx_lib.rpx_debug_encoder_gemm(site, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None)
+        assert rc == _native.RPX_ERR_CUDA and _native.last_error()
+    for site in (_native.RPX_EGEMM_OPROJ, _native.RPX_EGEMM_FFN_DOWN):
+        rc = rpx_lib.rpx_debug_encoder_gemm(site, 1, buf, buf, 4, 64, 128, 1e-6, None, None, buf, buf, buf, None, 0, None)
+        assert rc == _native.RPX_ERR_CUDA and _native.last_error()
     rc = rpx_lib.rpx_sim_topk(buf, 1, buf, 10, 64, 5, None, 0, buf, None, buf, None, 0, buf, 1024, None)
     assert rc != _native.RPX_OK
     rc = rpx_lib.rpx_topk_merge(buf, buf, 2, 1, 5, buf, None, buf, None, None)
@@ -87,6 +95,18 @@ def test_compute_fails_loudly_without_gpu(rpx_lib):
     h = C.c_void_p()
     rc = rpx_lib.rpx_index_create(buf, 4, 64, buf, None, C.byref(h))
     assert rc != _native.RPX_OK and not h.value
+
+
+@needs_no_gpu
+def test_encoder_gemm_entry_rejects_bad_input_before_touching_a_device(rpx_lib):
+    buf = (C.c_uint8 * 1024)()
+    call = rpx_lib.rpx_debug_encoder_gemm
+    assert call(4, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_QKV, 0, buf, buf, 4, 256, 64, 1e-6, None, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_OPROJ, 1, buf, buf, 4, 64, 64, 1e-6, None, None, buf, buf, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_QKV, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, buf, 64, None) == _native.RPX_ERR_INVALID
+    rc = call(_native.RPX_EGEMM_FFN_UP, 1, buf, buf, 4, 384, 64, 1e-6, buf, buf, None, None, None, None, 0, None)
+    assert rc == _native.RPX_ERR_UNSUPPORTED and "multiple of 256" in _native.last_error()
 
 
 @needs_no_gpu
