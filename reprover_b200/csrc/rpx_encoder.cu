@@ -27,10 +27,10 @@ namespace rpx {
 
 namespace {
 
-// Throughput-path tiles of QKV, O-proj and FFN-down: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand
-// ring fit the 227 KB of shared memory an H100 block may use.  The gated FFN up-projection runs on gemm_ws_kernel's
-// 128 x 256 tiles instead (rpx_gemm_ws.cuh): on an H100 it measured 12 % faster there, while the other three
-// GEMMs measured 6-18 % slower, their epilogues no longer overlapping the next tile's MMAs.
+// Throughput-path tiles of QKV: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand ring fit the 227 KB
+// of shared memory an H100 block may use.  The gated FFN up-projection, O-proj and FFN-down run on
+// gemm_ws_kernel's 128 x 256 tiles instead (rpx_gemm_ws.cuh); QKV measured 6 % slower there, its epilogue no
+// longer overlapping the next tile's MMAs.
 constexpr int kBlockN = 128;
 
 struct LayerW {
@@ -244,11 +244,9 @@ struct PdlScope {
   ~PdlScope() { set_pdl_scope(false); }
 };
 
-// RMSNorm partial sums per row: one per 128-wide n-tile on the throughput path, one per 32-column chunk on the
-// latency path.
-int ss_parts(int d_model, bool latency) {
-  return ceil_div(d_model, latency ? 32 : kBlockN) * (EpiResidual::kWarps / 4);
-}
+// RMSNorm partial sums per row: one per 128 columns on the throughput path (EpiWsResidual: two per 256-wide
+// tile), one per 32-column chunk on the latency path.
+int ss_parts(int d_model, bool latency) { return ceil_div(d_model, latency ? 32 : 128); }
 
 // The encoder's four GEMMs, each on the tiles the forward pass uses for T tokens on the throughput or the
 // latency path.  forward(), forward_latency_layer() and rpx_debug_encoder_gemm all launch through these, so the
@@ -266,21 +264,30 @@ int qkv_gemm(bool latency, int T, const void* A, const void* B, int N, int K, co
 }
 
 // h32 [T, N] += A B^T, h16 = bf16(h32), ss_out = partial sums of h32^2 ([ss_parts(N)][T]).
+// The throughput path runs gemm_ws_kernel with the residual block streamed into shared memory.  How its 227 KB
+// are split is chosen per site (RES_BUFS chunk buffers of 8 KB per consumer, STAGES operand stages of 48 KB), as
+// measured fastest at 2^18 tokens on an H100 80GB HBM3 at a 700 W power limit (tools/residual_gemm_bench.py):
+//   O-proj   (K = 384, 6 k-blocks): 4 stages and 2 chunk buffers.  It is memory-bound, and its A operand is a
+//            third of its HBM reads: the deep ring loads 4 of the next tile's 6 k-blocks while the epilogue
+//            runs.  3 stages and 5 buffers took 3 % longer, 2 stages and 7 buffers 4 %.
+//   FFN-down (K = 3584, 56 k-blocks): 3 stages and 5 chunk buffers.  With 2 buffers per consumer the epilogue
+//            waited on 3 residual round trips per tile and took 5 % longer.
+template <int RES_BUFS, int STAGES>
 int residual_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                   float* ss_out, cudaStream_t st) {
   EpiResidualParams ep{h32, h16, N, ss_out, T};
-  if (!latency) return launch_gemm<kBlockN, EpiResidual>(A, K, B, K, T, N, K, ep, st);
+  if (!latency) return launch_gemm_ws<EpiWsResidual<RES_BUFS>, STAGES>(A, K, B, K, T, N, K, ep, st);
   if (T <= kLatSmallMMaxTokens)
-    return launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st);
-  return launch_gemm<kLatBlockN, EpiResidualT<true>, false, kLatStages>(A, K, B, K, T, N, K, ep, st);
+    return launch_gemm<kLatBlockN, EpiResidualChunkSS, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st);
+  return launch_gemm<kLatBlockN, EpiResidualChunkSS, false, kLatStages>(A, K, B, K, T, N, K, ep, st);
 }
 int oproj_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                float* ss_out, cudaStream_t st) {
-  return residual_gemm(latency, T, A, B, N, K, h32, h16, ss_out, st);
+  return residual_gemm<2, 4>(latency, T, A, B, N, K, h32, h16, ss_out, st);
 }
 int ffn_down_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                   float* ss_out, cudaStream_t st) {
-  return residual_gemm(latency, T, A, B, N, K, h32, h16, ss_out, st);
+  return residual_gemm<5, 3>(latency, T, A, B, N, K, h32, h16, ss_out, st);
 }
 
 // out [T, N/2] = bf16(gelu_new(A B^T_gate * rs[m]) * (A B^T_linear * rs[m])).  B interleaves the gate and linear

@@ -487,10 +487,12 @@ struct EpiStoreBF16 {
   __device__ void finish() {}
 };
 
-// Residual update (attention output projection K8 and FFN down projection K9):
-//   h32[m, n] += acc;  h16[m, n] = bf16(h32[m, n]);  ss_out[part-of-n_blk][m] = sum_n h32[m, n]^2
+// Residual update (attention output projection K8 and FFN down projection K9) of the latency path:
+//   h32[m, n] += acc;  h16[m, n] = bf16(h32[m, n]);  ss_out[n / 32][m] = sum over the 32-column chunk of h32[m, n]^2
 // The fp32 copy is the residual stream; the bf16 copy is the next GEMM's A operand;
-// ss_out feeds the next RMSNorm (see RowScale).
+// ss_out feeds the next RMSNorm (see RowScale).  One partial sum per 32-column chunk: the latency path uses 32- or
+// 64-wide tiles depending on the token count and must hand the next RMSNorm the same partial sums either way.
+// The throughput path runs EpiWsResidual (rpx_gemm_ws.cuh).
 //
 // The accumulator arrives one ROW per thread, which is the worst possible layout for global
 // memory: a warp-wide 16-byte access would touch 32 different 128-byte lines.  Each warp
@@ -498,18 +500,14 @@ struct EpiStoreBF16 {
 // read-modify-write with lanes running along the row: one instruction covers 4 rows x 128
 // contiguous bytes (4 L1 wavefronts instead of 32).  Residual loads run one chunk ahead.
 // (RPX_EPI_WARPS=8 — two warps per lane group splitting the chunks — is off by default.)
-// CHUNK_SS: one partial sum per 32-column chunk instead of one per tile (ss_out is then indexed by the chunk's
-// position in the row, [N / 32][ss_stride]) — the latency path uses 32- or 64-wide tiles depending on the token
-// count and must hand the next RMSNorm the same partial sums either way.
 struct EpiResidualParams {
   float* h32;
   __nv_bfloat16* h16;
   int ld;
-  float* ss_out;  // [tiles_n * kWarps / 4][ss_stride]
+  float* ss_out;  // [n_parts][ss_stride], n_parts = ss_parts(ld, latency) of rpx_encoder.cu
   int ss_stride;
 };
-template <bool CHUNK_SS>
-struct EpiResidualT {
+struct EpiResidualChunkSS {
   using Params = EpiResidualParams;
   static constexpr int kWarps = RPX_EPI_WARPS;
   static constexpr size_t kSmemBytes = kWarps * 32 * 32 * sizeof(float);  // one 32x32 tile per warp
@@ -517,7 +515,7 @@ struct EpiResidualT {
   float4* stg;  // this warp's staging tile: row r = 8 float4, stored at slot (j ^ (r & 7))
   int lane, grp;
   float4 h[8];  // residual values of the chunk in flight (loaded one chunk ahead)
-  __device__ EpiResidualT(const Params& p_, uint8_t* smem_extra, int row, int part) : p(p_) {
+  __device__ EpiResidualChunkSS(const Params& p_, uint8_t* smem_extra, int row, int part) : p(p_) {
     lane = row & 31;
     grp = row >> 5;
     stg = reinterpret_cast<float4*>(smem_extra) + (part * 4 + grp) * 32 * 8;
@@ -580,13 +578,10 @@ struct EpiResidualT {
       __syncwarp();
 #pragma unroll
       for (int i = 0; i < 8; ++i) h[i] = hn[i];
-      if (CHUNK_SS) {
-        write_ss(t, ss, row_base, sub, (t.n0 + c) >> 5);
+      write_ss(t, ss, row_base, sub, (t.n0 + c) >> 5);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) ss[i] = 0.f;
-      }
+      for (int i = 0; i < 8; ++i) ss[i] = 0.f;
     }
-    if (!CHUNK_SS) write_ss(t, ss, row_base, sub, t.n_blk * t.split + t.part);
   }
   // a row's partial sums sit in the 8 lanes that share `sub`
   __device__ __forceinline__ void write_ss(const TileCtx& t, float (&ss)[8], int row_base, int sub, int part_idx) const {
@@ -602,7 +597,6 @@ struct EpiResidualT {
   }
   __device__ void finish() {}
 };
-using EpiResidual = EpiResidualT<false>;
 
 // gelu_new (tanh form) — HF activations.py NewGELUActivation, used by T5 "gated-gelu".
 __device__ __forceinline__ float gelu_new(float x) {

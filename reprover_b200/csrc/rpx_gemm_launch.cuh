@@ -49,9 +49,10 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
   return RPX_OK;
 }
 
-// Throughput core (gemm_ws_kernel): 128 x 256 tiles, persistent over one CTA per SM.
+// Throughput core (gemm_ws_kernel): 128 x 256 tiles, persistent over one CTA per SM, a STAGES-deep operand ring.
 // A: [M, K] bf16 (row pitch lda), B: [N, K] bf16 (row pitch ldb).  K % 64 == 0, N % 32 == 0.
-template <class Epi>
+// Residual epilogues (Epi::kResBufs > 0) stream ep.h32 ([M, N] fp32, row pitch ep.ld) through TMA.
+template <class Epi, int STAGES = 4>
 int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
                    const typename Epi::Params& ep, cudaStream_t stream) {
   RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
@@ -59,15 +60,19 @@ int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M
   RPX_REQUIRE(N % 32 == 0, RPX_ERR_UNSUPPORTED, "gemm: N=%d must be a multiple of 32", N);
   DeviceInfo dev;
   RPX_TRY(get_device_info(&dev));
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmR;
   RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, kBlockM));
   RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, kWsBlockN));
+  if constexpr (Epi::kResBufs > 0)
+    RPX_TRY(make_tmap_2d(&tmR, 4, ep.h32, (uint64_t)M, (uint64_t)N, (uint64_t)ep.ld, kResChunkCols, 64, 128));
+  else
+    tmR = tmA;  // not read
   const int tiles_m = ceil_div(M, kBlockM);
   const int tiles_n = ceil_div(N, kWsBlockN);
-  const size_t smem = WsCfg::kSmemBytes;
+  const size_t smem = WsCfg<STAGES, Epi::kResBufs>::kSmemBytes;
   RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu", smem,
               dev.smem_optin);
-  auto kern = gemm_ws_kernel<Epi>;
+  auto kern = gemm_ws_kernel<Epi, STAGES>;
   static thread_local int configured_dev = -1;  // per-instantiation, per-thread
   if (configured_dev != dev.device) {
     RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -75,8 +80,8 @@ int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M
   }
   int grid = tiles_m * tiles_n;
   if (grid > dev.num_sms) grid = dev.num_sms;
-  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA, tmB, M, N, K, tiles_m,
-                         tiles_n, ep));
+  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA, tmB, tmR, M, N, K,
+                         tiles_m, tiles_n, ep));
   return RPX_OK;
 }
 

@@ -4,10 +4,15 @@
 //   D[M, N] (fp32) = A[M, K] * B[N, K]^T        A, B bf16, K contiguous, K % 64 == 0
 //
 // Structure (one persistent CTA per SM, 384 threads, tiles visited n-fastest like gemm_tc_kernel):
-//   warpgroup 0     : TMA producer — one elected thread streams 128 x 64 A and 256 x 64 B tiles into a 4-deep
+//   warpgroup 0     : TMA producers, which give their registers away (setmaxnreg.dec to 40).
+//                     warp 0: one elected thread streams 128 x 64 A and 256 x 64 B tiles into a STAGES-deep
 //                     128B-swizzled ring (48 KB per stage), completion on `full[]`.  It keeps filling the ring
 //                     across tile boundaries, so the next tile's first k-blocks land while the consumers run the
-//                     epilogue.  The warpgroup gives its registers away (setmaxnreg.dec to 40).
+//                     epilogue.
+//                     warps 1, 2 (residual epilogues, Epi::kResBufs > 0): warp 1 + w streams the fp32 residual
+//                     block of consumer w's rows into that consumer's ring of kResBufs chunk buffers (64 rows x
+//                     32 columns, 8 KB, 128B-swizzled), completion on `rfull[]`, released on `rempty[]`.  A tile's
+//                     chunks are requested as soon as a buffer is free, i.e. while its mainloop still runs.
 //   warpgroups 1, 2 : consumers — consumer w owns rows [64w, 64w + 64) of the tile and issues wgmma.m64n256k16
 //                     (128 fp32 accumulator registers per thread, setmaxnreg.inc to 232); a stage goes back to
 //                     the producer (`empty[]`) once the wgmma group that read it has retired.  After the last
@@ -16,7 +21,12 @@
 // Against gemm_tc_kernel (128 x 128 tiles, accumulator handed to epilogue warps through a 66 KB shared-memory
 // tile): a k-block brings 48 KB for 4.2 MFLOP instead of 32 KB for 2.1 MFLOP, every m64n256k16 reads its A
 // slice once per 256 columns, and no shared memory is held for the hand-off.  The epilogue no longer overlaps
-// the MMAs of the next tile inside the CTA; its global reads are started early instead (Epi::prefetch).
+// the MMAs of the next tile inside the CTA, so no epilogue thread waits on a global load: what the epilogue
+// reads either arrives in shared memory ahead of it (the residual stream) or is fetched during the first
+// k-block (Epi::prefetch).
+//
+// Shared memory: STAGES x 48 KB of operand ring + 2 x kResBufs x 8 KB of residual chunks within the 227 KB an
+// H100 block may use; the residual GEMMs choose the split per site (rpx_encoder.cu, residual_gemm).
 //
 // Fragment layout (rpx_ptx.cuh): the thread with lane l of warp v (0..3) of consumer w holds rows
 // r0 = 64w + 16v + l/4 and r0 + 8 of the tile; acc[4j], acc[4j+1] are row r0, columns 8j + 2(l%4) + {0, 1}, and
@@ -28,15 +38,20 @@
 namespace rpx {
 
 constexpr int kWsBlockN = 256;
-constexpr int kWsStages = 4;
 constexpr int kWsThreads = 384;
+constexpr int kResChunkCols = 32;                                  // one 128-byte swizzle row of fp32
+constexpr int kResChunkBytes = 64 * kResChunkCols * 4;             // 8 KB: a consumer's 64 rows
 
+template <int STAGES, int RES_BUFS>
 struct WsCfg {
+  static_assert(2 * STAGES + 4 * RES_BUFS <= 32, "barrier block holds 32 mbarriers");
   static constexpr int kABytes = kBlockM * kBlockK * 2;    // 16 KB
   static constexpr int kBBytes = kWsBlockN * kBlockK * 2;  // 32 KB
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // ring + 1 KB alignment slack + barriers
-  static constexpr size_t kSmemBytes = (size_t)kWsStages * kStageBytes + 1024 + 256;
+  static constexpr int kRingBytes = STAGES * kStageBytes;
+  static constexpr int kResBytes = 2 * RES_BUFS * kResChunkBytes;
+  // ring + residual chunks + 1 KB alignment slack + barriers
+  static constexpr size_t kSmemBytes = (size_t)kRingBytes + kResBytes + 1024 + 256;
 };
 
 // What a register-fragment epilogue sees for one output tile.
@@ -49,24 +64,43 @@ struct FragCtx {
   int q;       // lane % 4: this thread's columns are 8j + 2q + {0, 1}
 };
 
+// This consumer's ring of residual chunk buffers (Epi::kResBufs > 0).  Chunk k of a tile is columns
+// [32k, 32k + 32) of the consumer's 64 rows; 16-byte unit u of row r sits at unit u ^ (r % 8) of that row
+// (TMA 128B swizzle).  The chunks of successive tiles take the buffers in turn.
+struct ResStream {
+  float* buf;       // kResBufs x 64 x 32 fp32
+  uint64_t* full;   // kResBufs mbarriers: the producer's TMA landed
+  uint64_t* empty;  // kResBufs mbarriers: all 128 consumer threads are done with the buffer
+};
+
 // Epi must provide:
 //   struct Params;                                  (trivially copyable kernel argument)
-//   __device__ explicit Epi(const Params&);
+//   static constexpr int kResBufs;                  (residual chunk buffers per consumer; 0: no residual stream)
+//   __device__ Epi(const Params&, const ResStream&);
 //   __device__ void prefetch(const FragCtx&);       (runs while the tile's first k-block is in flight: global
 //                                                    reads that do not depend on the accumulator)
 //   __device__ void tile(const FragCtx&, const float (&acc)[128]);
-template <class Epi>
+// With kResBufs > 0, tmR maps the residual matrix ([M, N] fp32, box 32 x 64, 128B swizzle): the producer loads,
+// for every tile and consumer whose first row is < M, the chunks k with 32k < n_cols in order, and tile() must
+// consume exactly those.
+template <class Epi, int STAGES>
 __global__ void __launch_bounds__(kWsThreads, 1)
-gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
-               int tiles_m, int tiles_n, typename Epi::Params ep) {
+gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmR, int M, int N, int K, int tiles_m, int tiles_n,
+               typename Epi::Params ep) {
+  using Cfg = WsCfg<STAGES, Epi::kResBufs>;
+  constexpr int R = Epi::kResBufs;
   extern __shared__ uint8_t smem_raw[];
   // 128B swizzle needs 1024-byte aligned tile bases.
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024 - (raw_addr & 1023)) & 1023);
   uint8_t* sA = smem;
-  uint8_t* sB = smem + kWsStages * WsCfg::kABytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kWsStages * WsCfg::kStageBytes);
-  uint64_t* empty = full + kWsStages;
+  uint8_t* sB = smem + STAGES * Cfg::kABytes;
+  float* sR = reinterpret_cast<float*>(smem + Cfg::kRingBytes);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::kRingBytes + Cfg::kResBytes);
+  uint64_t* empty = full + STAGES;
+  uint64_t* rfull = empty + STAGES;  // [2][R]
+  uint64_t* rempty = rfull + 2 * R;  // [2][R]
 
   const int warp = threadIdx.x >> 5;
   const int wg = warp >> 2;
@@ -76,9 +110,14 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < kWsStages; ++s) {
+    if (R > 0) tma_prefetch_desc(&tmR);
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 2 * 128);  // every thread of both consumers
+    }
+    for (int s = 0; s < 2 * R; ++s) {
+      mbar_init(&rfull[s], 1);
+      mbar_init(&rempty[s], 128);  // every thread of the consumer
     }
     fence_mbar_init();
   }
@@ -89,20 +128,43 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_wait();
 
   if (wg == 0) {
-    // ------------------------------------------------------------------ TMA producer
     setmaxnreg_dec<40>();
     if (warp == 0 && elect_one()) {
+      // ---------------------------------------------------------------- TMA producer: operands
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const int m_blk = t / tiles_n, n_blk = t % tiles_n;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full[stage], WsCfg::kStageBytes);
-          tma_load_2d(sA + stage * WsCfg::kABytes, &tmA, &full[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sB + stage * WsCfg::kBBytes, &tmB, &full[stage], kb * kBlockK, n_blk * kWsBlockN);
-          if (++stage == kWsStages) {
+          mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
+          tma_load_2d(sA + stage * Cfg::kABytes, &tmA, &full[stage], kb * kBlockK, m_blk * kBlockM);
+          tma_load_2d(sB + stage * Cfg::kBBytes, &tmB, &full[stage], kb * kBlockK, n_blk * kWsBlockN);
+          if (++stage == STAGES) {
             stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    } else if (R > 0 && (warp == 1 || warp == 2) && elect_one()) {
+      // ---------------------------------------------------------------- TMA producer: residual chunks
+      const int w = warp - 1;  // consumer served
+      float* buf = sR + w * R * (kResChunkBytes / 4);
+      uint64_t* rf = rfull + w * R;
+      uint64_t* re = rempty + w * R;
+      int b = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int row0 = (t / tiles_n) * kBlockM + 64 * w;
+        const int n0 = (t % tiles_n) * kWsBlockN;
+        const int n_cols = N - n0 < kWsBlockN ? N - n0 : kWsBlockN;
+        if (row0 >= M) continue;
+        for (int col = 0; col < n_cols; col += kResChunkCols) {
+          mbar_wait(&re[b], phase ^ 1);
+          mbar_arrive_expect_tx(&rf[b], kResChunkBytes);  // rows past M arrive zero-filled and count in full
+          tma_load_2d(buf + b * (kResChunkBytes / 4), &tmR, &rf[b], n0 + col, row0);
+          if (++b == R) {
+            b = 0;
             phase ^= 1;
           }
         }
@@ -113,7 +175,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     setmaxnreg_inc<232>();
     const int cw = wg - 1;  // which 64-row half of the tile
     const int lane = threadIdx.x & 31;
-    Epi epi(ep);
+    Epi epi(ep, ResStream{sR + cw * R * (kResChunkBytes / 4), rfull + cw * R, rempty + cw * R});
     float acc[128];
     int stage = 0;
     uint32_t phase = 0;
@@ -131,8 +193,8 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
         // +8 KB (>>4 = 512) for the second 64-row half of A; +32 bytes (>>4 = 2) per K=16 step inside the atom
-        const uint64_t a_desc = make_smem_desc_kmajor_sw128(smem_u32(sA + stage * WsCfg::kABytes)) + 512 * cw;
-        const uint64_t b_desc = make_smem_desc_kmajor_sw128(smem_u32(sB + stage * WsCfg::kBBytes));
+        const uint64_t a_desc = make_smem_desc_kmajor_sw128(smem_u32(sA + stage * Cfg::kABytes)) + 512 * cw;
+        const uint64_t b_desc = make_smem_desc_kmajor_sw128(smem_u32(sB + stage * Cfg::kBBytes));
         wgmma_fence_operand(acc);
         wgmma_fence();
 #pragma unroll
@@ -145,7 +207,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_arrive(&empty[prev]);
         }
         prev = stage;
-        if (++stage == kWsStages) {
+        if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
@@ -164,8 +226,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // C[m, n] = acc (fp32).  The bare core behind rpx_gemm_bf16_f32.
 struct EpiWsStoreF32 {
   using Params = EpiStoreF32::Params;
+  static constexpr int kResBufs = 0;
   Params p;
-  __device__ explicit EpiWsStoreF32(const Params& p_) : p(p_) {}
+  __device__ EpiWsStoreF32(const Params& p_, const ResStream&) : p(p_) {}
   __device__ void prefetch(const FragCtx&) {}
   __device__ void tile(const FragCtx& c, const float (&acc)[128]) {
 #pragma unroll
@@ -189,9 +252,10 @@ struct EpiWsGeGLU {
     int ldo;
     RowScale rs;
   };
+  static constexpr int kResBufs = 0;
   Params p;
   float rs0 = 0.f, rs1 = 0.f;
-  __device__ explicit EpiWsGeGLU(const Params& p_) : p(p_) {}
+  __device__ EpiWsGeGLU(const Params& p_, const ResStream&) : p(p_) {}
   __device__ void prefetch(const FragCtx& c) {
     rs0 = c.r0 < c.M ? p.rs.get(c.r0) : 0.f;
     rs1 = c.r0 + 8 < c.M ? p.rs.get(c.r0 + 8) : 0.f;
@@ -208,6 +272,97 @@ struct EpiWsGeGLU {
       if (c.r0 + 8 < c.M)
         *reinterpret_cast<uint32_t*>(dst + 8 * (size_t)p.ldo + 8 * j) =
             pack_bf16x2(gelu_new(g[2] * rs1) * (u[2] * rs1), gelu_new(g[3] * rs1) * (u[3] * rs1));
+    }
+  }
+};
+
+// Residual update of the throughput path (attention output projection K8, FFN down projection K9):
+//   h32[m, n] += acc;  h16[m, n] = bf16(h32[m, n]);  ss_out[2 n_blk + n / 128 % 2][m] = sum over the 128-column
+//   half-tile of h32[m, n]^2
+// i.e. one RMSNorm partial sum per 128 columns, the layout ss_parts(D, false) describes.  The residual block
+// arrives in shared memory through the ResStream (RES_BUFS chunk buffers per consumer), so the epilogue never
+// waits on a global load.  Per 32-column chunk, warp v of the consumer (fragment rows [16v, 16v + 16)):
+//   1. adds its accumulator fragment into the chunk in place (h32 + acc, as EpiResidualChunkSS);
+//   2. reads its 16 rows back with lanes along the row — lane (s, j) takes float4 j of rows s, s + 4, s + 8,
+//      s + 12 — and writes h32 and h16 with 16- and 8-byte stores, 4 rows x 128 contiguous bytes per instruction;
+//   3. fences its shared-memory writes against the async proxy (the buffer's next TMA fill) and releases it.
+// Each lane sums its float4's squares over the half-tile's chunks in column order and a xor-1/2/4 shuffle adds
+// the 8 lanes of a row (within a chunk, the order of EpiResidualChunkSS): a fixed order that depends on neither
+// T nor the row's tile, so h32, h16 and the partial sums of a row are the same bits in every call.
+template <int RES_BUFS>
+struct EpiWsResidual {
+  using Params = EpiResidualParams;
+  static constexpr int kResBufs = RES_BUFS;
+  Params p;
+  ResStream rs;
+  int b = 0;           // buffer of the next chunk
+  uint32_t phase = 0;  // its rfull parity
+  __device__ EpiWsResidual(const Params& p_, const ResStream& rs_) : p(p_), rs(rs_) {}
+  __device__ void prefetch(const FragCtx&) {}
+  __device__ void tile(const FragCtx& c, const float (&acc)[128]) {
+    const int lane = threadIdx.x & 31;
+    const int v = (threadIdx.x >> 5) & 3;
+    const int row0 = c.r0 - 16 * v - (lane >> 2);  // first row of this consumer's 64
+    if (row0 >= c.M) return;                        // (the producer loads nothing for it either)
+    const int sub = lane >> 3, j4 = lane & 7;
+    float ss[4];
+#pragma unroll
+    for (int k = 0; k < kWsBlockN / kResChunkCols; ++k) {
+      if (kResChunkCols * k >= c.n_cols) break;
+      if (k % 4 == 0) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ss[i] = 0.f;
+      }
+      float* s = rs.buf + b * (kResChunkBytes / 4);
+      mbar_wait(&rs.full[b], phase);
+      // 1. fragment columns 8jj + 2q + {0, 1} of rows 16v + lane/4 (+ 8)
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * k + jj;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = 16 * v + (lane >> 2) + 8 * h;
+          float2* x = reinterpret_cast<float2*>(s + r * kResChunkCols + (((2 * jj + (c.q >> 1)) ^ (r & 7)) << 2) + 2 * (c.q & 1));
+          float2 hv = *x;
+          hv.x += acc[4 * j + 2 * h];
+          hv.y += acc[4 * j + 2 * h + 1];
+          *x = hv;
+        }
+      }
+      __syncwarp();
+      // 2. rows along the lanes
+      const size_t col = (size_t)c.n0 + kResChunkCols * k + 4 * j4;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int r = 16 * v + sub + 4 * i;
+        const int m = row0 + r;
+        const float4 hv = *reinterpret_cast<const float4*>(s + r * kResChunkCols + ((j4 ^ (r & 7)) << 2));
+        ss[i] += hv.x * hv.x + hv.y * hv.y + hv.z * hv.z + hv.w * hv.w;
+        if (m < c.M) {
+          *reinterpret_cast<float4*>(p.h32 + (size_t)m * p.ld + col) = hv;
+          *reinterpret_cast<uint2*>(p.h16 + (size_t)m * p.ld + col) =
+              make_uint2(pack_bf16x2(hv.x, hv.y), pack_bf16x2(hv.z, hv.w));
+        }
+      }
+      // 3. the buffer goes back to the producer
+      fence_proxy_async_smem();
+      mbar_arrive(&rs.empty[b]);
+      if (++b == RES_BUFS) {
+        b = 0;
+        phase ^= 1;
+      }
+      if (k % 4 == 3 || kResChunkCols * (k + 1) >= c.n_cols) {
+        const int part = 2 * c.n_blk + k / 4;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          float t = ss[i];
+          t += __shfl_xor_sync(0xffffffffu, t, 1);
+          t += __shfl_xor_sync(0xffffffffu, t, 2);
+          t += __shfl_xor_sync(0xffffffffu, t, 4);
+          const int m = row0 + 16 * v + sub + 4 * i;
+          if (j4 == 0 && m < c.M) p.ss_out[(size_t)part * p.ss_stride + m] = t;
+        }
+      }
     }
   }
 };
