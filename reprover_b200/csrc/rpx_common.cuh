@@ -77,19 +77,31 @@ unsigned long long* next_timeline_slot();
 bool pdl_enabled();
 void set_pdl_scope(bool on);  // per thread: true while such a forward enqueues its kernels
 
-// Kernel launch with (optionally) the programmatic-stream-serialization attribute; see rpx_ptx.cuh.
-template <typename Kern, typename... Args>
+// Kernel launch with (optionally) the programmatic-stream-serialization attribute; see rpx_ptx.cuh.  CLUSTER > 1
+// launches clusters of that many CTAs along x (grid.x must be a multiple of it).
+template <int CLUSTER = 1, typename Kern, typename... Args>
 inline cudaError_t launch_pdl(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute at[2];
+  int n = 0;
+  if (CLUSTER > 1) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = CLUSTER;
+    at[n].val.clusterDim.y = 1;
+    at[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (pdl) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = at;
-  cfg.numAttrs = pdl ? 1 : 0;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 

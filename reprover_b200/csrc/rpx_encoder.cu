@@ -266,40 +266,48 @@ int qkv_gemm(bool latency, int T, const void* A, const void* B, int N, int K, co
 // h32 [T, N] += A B^T, h16 = bf16(h32), ss_out = partial sums of h32^2 ([ss_parts(N)][T]).
 // The throughput path runs gemm_ws_kernel with the residual block streamed into shared memory.  How its 227 KB
 // are split is chosen per site (RES_BUFS chunk buffers of 8 KB per consumer, STAGES operand stages of 48 KB), as
-// measured fastest at 2^18 tokens on an H100 80GB HBM3 at a 700 W power limit (tools/residual_gemm_bench.py):
+// measured fastest at 2^18 tokens on an H100 80GB HBM3 at a 700 W power limit (tools/encoder_gemm_bench.py):
 //   O-proj   (K = 384, 6 k-blocks): 4 stages and 2 chunk buffers.  It is memory-bound, and its A operand is a
 //            third of its HBM reads: the deep ring loads 4 of the next tile's 6 k-blocks while the epilogue
 //            runs.  3 stages and 5 buffers took 3 % longer, 2 stages and 7 buffers 4 %.
 //   FFN-down (K = 3584, 56 k-blocks): 3 stages and 5 chunk buffers.  With 2 buffers per consumer the epilogue
 //            waited on 3 residual round trips per tile and took 5 % longer.
-template <int RES_BUFS, int STAGES>
+// CLUSTER is chosen the same way, on an H100 80GB HBM3 at a 400 W power limit (alternated runs of both forms):
+//   O-proj   unclustered: 1.81-1.92 ms against 1.90-1.96 ms as pairs.  Being HBM-bound, it gains nothing from the
+//            lower L2 traffic and pays for the coupling of the pair.  Its split as pairs (3 stages, 5 buffers)
+//            took 1.85-1.96 ms.
+//   FFN-down pairs: 6.31-6.44 ms against 6.38-6.59 ms unclustered.  As pairs, 4 stages and 2 buffers took
+//            6.50-6.58 ms, so the split stays.
+template <int RES_BUFS, int STAGES, int CLUSTER>
 int residual_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                   float* ss_out, cudaStream_t st) {
   EpiResidualParams ep{h32, h16, N, ss_out, T};
-  if (!latency) return launch_gemm_ws<EpiWsResidual<RES_BUFS>, STAGES>(A, K, B, K, T, N, K, ep, st);
+  if (!latency) return launch_gemm_ws<EpiWsResidual<RES_BUFS>, STAGES, CLUSTER>(A, K, B, K, T, N, K, ep, st);
   if (T <= kLatSmallMMaxTokens)
     return launch_gemm<kLatBlockN, EpiResidualChunkSS, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st);
   return launch_gemm<kLatBlockN, EpiResidualChunkSS, false, kLatStages>(A, K, B, K, T, N, K, ep, st);
 }
 int oproj_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                float* ss_out, cudaStream_t st) {
-  return residual_gemm<2, 4>(latency, T, A, B, N, K, h32, h16, ss_out, st);
+  return residual_gemm<2, 4, 1>(latency, T, A, B, N, K, h32, h16, ss_out, st);
 }
 int ffn_down_gemm(bool latency, int T, const void* A, const void* B, int N, int K, float* h32, __nv_bfloat16* h16,
                   float* ss_out, cudaStream_t st) {
-  return residual_gemm<5, 3>(latency, T, A, B, N, K, h32, h16, ss_out, st);
+  return residual_gemm<5, 3, 2>(latency, T, A, B, N, K, h32, h16, ss_out, st);
 }
 
 // out [T, N/2] = bf16(gelu_new(A B^T_gate * rs[m]) * (A B^T_linear * rs[m])).  B interleaves the gate and linear
 // rows in 128-row blocks (rpx_encoder_create), and every tile pairs gate column j with linear column j + 128 of
 // its 256-row block, so N must be a whole number of such blocks.
+// The throughput path runs the core as pairs (kFfnUpCluster): at 2^18 tokens on an H100 80GB HBM3 at a 400 W power
+// limit they took 11.60-11.87 ms against 12.61-12.70 ms unclustered (cuBLAS: 10.4-10.7 ms, tools/gemm_bench.py).
 int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K, const RowScale& rs,
                 __nv_bfloat16* out, cudaStream_t st) {
   RPX_REQUIRE(N % 256 == 0, RPX_ERR_UNSUPPORTED, "ffn-up gemm: N=%d must be a multiple of 256 (2 x d_ff, d_ff %% 128 == 0)", N);
   const int F = N / 2;
   if (!latency) {
     EpiWsGeGLU::Params ep{out, F, rs};
-    return launch_gemm_ws<EpiWsGeGLU>(A, K, B, K, T, N, K, ep, st);
+    return launch_gemm_ws<EpiWsGeGLU, kFfnUpStages, kFfnUpCluster>(A, K, B, K, T, N, K, ep, st);
   }
   // hidden units per tile: 32 (64-column tiles, T <= 128: 112 CTAs) or 64 (128-column tiles: 56 x ceil(T/128))
   if (T <= kBlockM) {

@@ -7,7 +7,8 @@ extern "C" int rpx_gemm_bf16_f32(const void* d_A, const void* d_B, float* d_C, i
   using namespace rpx;
   RPX_REQUIRE(d_A && d_B && d_C, RPX_ERR_INVALID, "rpx_gemm_bf16_f32: null pointer");
   EpiWsStoreF32::Params ep{d_C, N};
-  return launch_gemm_ws<EpiWsStoreF32>(d_A, K, d_B, K, M, N, K, ep, static_cast<cudaStream_t>(stream));
+  return launch_gemm_ws<EpiWsStoreF32, kFfnUpStages, kFfnUpCluster>(d_A, K, d_B, K, M, N, K, ep,
+                                                                   static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int rpx_gemm1_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N, int32_t K,

@@ -49,10 +49,16 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
   return RPX_OK;
 }
 
-// Throughput core (gemm_ws_kernel): 128 x 256 tiles, persistent over one CTA per SM, a STAGES-deep operand ring.
+// The form of the throughput core the FFN up-projection runs (rpx_encoder.cu, ffn_up_gemm), which the bare entry
+// rpx_gemm_bf16_f32 runs as well.
+constexpr int kFfnUpStages = 4;
+constexpr int kFfnUpCluster = 2;
+
+// Throughput core (gemm_ws_kernel): 128 x 256 tiles, persistent over one CTA per SM, a STAGES-deep operand ring;
+// CLUSTER = 2 runs clusters of two CTAs on vertically adjacent tiles that share the B tile by TMA multicast.
 // A: [M, K] bf16 (row pitch lda), B: [N, K] bf16 (row pitch ldb).  K % 64 == 0, N % 32 == 0.
 // Residual epilogues (Epi::kResBufs > 0) stream ep.h32 ([M, N] fp32, row pitch ep.ld) through TMA.
-template <class Epi, int STAGES = 4>
+template <class Epi, int STAGES, int CLUSTER>
 int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
                    const typename Epi::Params& ep, cudaStream_t stream) {
   RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
@@ -62,7 +68,8 @@ int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M
   RPX_TRY(get_device_info(&dev));
   CUtensorMap tmA, tmB, tmR;
   RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, kBlockM));
-  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, kWsBlockN));
+  // (each CTA of a pair loads one half of the B tile)
+  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, kWsBlockN / CLUSTER));
   if constexpr (Epi::kResBufs > 0)
     RPX_TRY(make_tmap_2d(&tmR, 4, ep.h32, (uint64_t)M, (uint64_t)N, (uint64_t)ep.ld, kResChunkCols, 64, 128));
   else
@@ -72,16 +79,31 @@ int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M
   const size_t smem = WsCfg<STAGES, Epi::kResBufs>::kSmemBytes;
   RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu", smem,
               dev.smem_optin);
-  auto kern = gemm_ws_kernel<Epi, STAGES>;
+  auto kern = gemm_ws_kernel<Epi, STAGES, CLUSTER>;
   static thread_local int configured_dev = -1;  // per-instantiation, per-thread
+  static thread_local int max_clusters = 0;     // co-resident clusters of this instantiation on that device
   if (configured_dev != dev.device) {
     RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(CLUSTER * dev.num_sms);
+    cfg.blockDim = dim3(kWsThreads);
+    cfg.dynamicSmemBytes = smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = CLUSTER;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    RPX_CUDA_OK(cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg));
+    RPX_REQUIRE(max_clusters > 0, RPX_ERR_UNSUPPORTED, "gemm: no cluster of %d CTAs with %zu B smem fits the device",
+                CLUSTER, smem);
     configured_dev = dev.device;
   }
-  int grid = tiles_m * tiles_n;
-  if (grid > dev.num_sms) grid = dev.num_sms;
-  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA, tmB, tmR, M, N, K,
-                         tiles_m, tiles_n, ep));
+  int clusters = ceil_div(tiles_m, CLUSTER) * tiles_n;  // work units
+  if (clusters > max_clusters) clusters = max_clusters;
+  RPX_CUDA_OK(launch_pdl<CLUSTER>(kern, dim3(CLUSTER * clusters), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA,
+                                  tmB, tmR, M, N, K, tiles_m, tiles_n, ep));
   return RPX_OK;
 }
 

@@ -8,16 +8,27 @@
 //                     warp 0: one elected thread streams 128 x 64 A and 256 x 64 B tiles into a STAGES-deep
 //                     128B-swizzled ring (48 KB per stage), completion on `full[]`.  It keeps filling the ring
 //                     across tile boundaries, so the next tile's first k-blocks land while the consumers run the
-//                     epilogue.
+//                     epilogue.  With CLUSTER = 2 (see below) it loads its own A tile and one half of the shared
+//                     B tile, which it multicasts into both CTAs.
 //                     warps 1, 2 (residual epilogues, Epi::kResBufs > 0): warp 1 + w streams the fp32 residual
 //                     block of consumer w's rows into that consumer's ring of kResBufs chunk buffers (64 rows x
 //                     32 columns, 8 KB, 128B-swizzled), completion on `rfull[]`, released on `rempty[]`.  A tile's
 //                     chunks are requested as soon as a buffer is free, i.e. while its mainloop still runs.
 //   warpgroups 1, 2 : consumers — consumer w owns rows [64w, 64w + 64) of the tile and issues wgmma.m64n256k16
 //                     (128 fp32 accumulator registers per thread, setmaxnreg.inc to 232); a stage goes back to
-//                     the producer (`empty[]`) once the wgmma group that read it has retired.  After the last
-//                     k-block each consumer runs the epilogue functor on its own fragment.
+//                     the producer (`empty[]`) once the wgmma group that read it has retired: lane 0 of each
+//                     consumer warp arrives once for its warp.  After the last k-block each consumer runs the
+//                     epilogue functor on its own fragment.
 //
+// CLUSTER = 2: the CTAs run as clusters of two on vertically adjacent tiles.  A work unit is an (m-tile pair,
+// n-tile), units visited n-fastest; rank r of the cluster takes m-tile 2 (u / tiles_n) + r.  Both need the same
+// 256 x 64 B tile per k-block, so rank r loads its rows [128r, 128r + 128) once from L2 and multicasts them
+// into the same offset of both CTAs' stage (tmB encoded with a 128-row box): a CTA pulls 32 KB per k-block
+// through L2 instead of 48 KB.  The B tile in shared memory is laid out as with CLUSTER = 1.  Since a refill
+// writes into the peer's shared memory, a stage goes back to the producer only once the consumer warps of both
+// CTAs have released it (each warp also arrives on the peer's `empty[]`).  When tiles_m is odd, the last pair's
+// rank-1 tile lies wholly past M: that CTA still runs the pipeline (TMA zero-fills its A and counts the full
+// box), and its epilogues store nothing.
 // Against gemm_tc_kernel (128 x 128 tiles, accumulator handed to epilogue warps through a 66 KB shared-memory
 // tile): a k-block brings 48 KB for 4.2 MFLOP instead of 32 KB for 2.1 MFLOP, every m64n256k16 reads its A
 // slice once per 256 columns, and no shared memory is held for the hand-off.  The epilogue no longer overlaps
@@ -83,11 +94,12 @@ struct ResStream {
 // With kResBufs > 0, tmR maps the residual matrix ([M, N] fp32, box 32 x 64, 128B swizzle): the producer loads,
 // for every tile and consumer whose first row is < M, the chunks k with 32k < n_cols in order, and tile() must
 // consume exactly those.
-template <class Epi, int STAGES>
+template <class Epi, int STAGES, int CLUSTER>
 __global__ void __launch_bounds__(kWsThreads, 1)
 gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmR, int M, int N, int K, int tiles_m, int tiles_n,
                typename Epi::Params ep) {
+  static_assert(CLUSTER == 1 || CLUSTER == 2, "one CTA, or a pair sharing the B tile");
   using Cfg = WsCfg<STAGES, Epi::kResBufs>;
   constexpr int R = Epi::kResBufs;
   extern __shared__ uint8_t smem_raw[];
@@ -105,7 +117,12 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int wg = warp >> 2;
   const int num_kb = K / kBlockK;
-  const int num_tiles = tiles_m * tiles_n;
+  // Work units: tiles (CLUSTER = 1) or vertically adjacent tile pairs; this CTA takes units u0, u0 + u_step, ...
+  const int rank = CLUSTER > 1 ? (int)cluster_ctarank() : 0;
+  const int num_units = (tiles_m + CLUSTER - 1) / CLUSTER * tiles_n;
+  const int u0 = (int)blockIdx.x / CLUSTER;
+  const int u_step = (int)gridDim.x / CLUSTER;
+  auto unit_m = [&](int u) { return CLUSTER * (u / tiles_n) + rank; };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -113,7 +130,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (R > 0) tma_prefetch_desc(&tmR);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 2 * 128);  // every thread of both consumers
+      mbar_init(&empty[s], CLUSTER * 8);  // every consumer warp of every CTA of the cluster
     }
     for (int s = 0; s < 2 * R; ++s) {
       mbar_init(&rfull[s], 1);
@@ -122,6 +139,8 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     fence_mbar_init();
   }
   __syncthreads();
+  // the peer's barriers are initialised before anything multicasts into this CTA or arrives on them
+  if (CLUSTER > 1) cluster_sync_all();
   // Under programmatic dependent launch (rpx_ptx.cuh) the preceding kernel may still be running: A, the row
   // scales and the residual stream are its outputs.
   pdl_launch_dependents();
@@ -133,13 +152,20 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // ---------------------------------------------------------------- TMA producer: operands
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int m_blk = t / tiles_n, n_blk = t % tiles_n;
+      for (int u = u0; u < num_units; u += u_step) {
+        const int m_blk = unit_m(u), n_blk = u % tiles_n;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
+          // with CLUSTER = 2 the peer's half of B completes on this barrier too
           mbar_arrive_expect_tx(&full[stage], Cfg::kStageBytes);
           tma_load_2d(sA + stage * Cfg::kABytes, &tmA, &full[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sB + stage * Cfg::kBBytes, &tmB, &full[stage], kb * kBlockK, n_blk * kWsBlockN);
+          if constexpr (CLUSTER == 1) {
+            tma_load_2d(sB + stage * Cfg::kBBytes, &tmB, &full[stage], kb * kBlockK, n_blk * kWsBlockN);
+          } else {
+            constexpr int H = kWsBlockN / 2;
+            tma_load_2d_multicast(sB + stage * Cfg::kBBytes + rank * H * kBlockK * 2, &tmB, &full[stage], kb * kBlockK,
+                                  n_blk * kWsBlockN + rank * H, (uint16_t)0x3);
+          }
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
@@ -154,9 +180,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       uint64_t* re = rempty + w * R;
       int b = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int row0 = (t / tiles_n) * kBlockM + 64 * w;
-        const int n0 = (t % tiles_n) * kWsBlockN;
+      for (int u = u0; u < num_units; u += u_step) {
+        const int row0 = unit_m(u) * kBlockM + 64 * w;
+        const int n0 = (u % tiles_n) * kWsBlockN;
         const int n_cols = N - n0 < kWsBlockN ? N - n0 : kWsBlockN;
         if (row0 >= M) continue;
         for (int col = 0; col < n_cols; col += kResChunkCols) {
@@ -179,10 +205,19 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     float acc[128];
     int stage = 0;
     uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    // One arrival per warp (lane 0, once the warp's wgmma_wait has returned in every lane), on this CTA's
+    // barrier and, with CLUSTER = 2, on the peer's.
+    auto release = [&](int st) {
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty[st]);
+        if (CLUSTER > 1) mbar_arrive_cluster(&empty[st], (uint32_t)(rank ^ 1));
+      }
+    };
+    for (int u = u0; u < num_units; u += u_step) {
       FragCtx c;
-      c.n_blk = t % tiles_n;
-      c.m0 = (t / tiles_n) * kBlockM;
+      c.n_blk = u % tiles_n;
+      c.m0 = unit_m(u) * kBlockM;
       c.n0 = c.n_blk * kWsBlockN;
       c.n_cols = N - c.n0 < kWsBlockN ? N - c.n0 : kWsBlockN;
       c.M = M;
@@ -204,7 +239,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // the group of the previous k-block has retired once at most this one is in flight: its stage is free
         if (kb > 0) {
           wgmma_wait<1>();
-          mbar_arrive(&empty[prev]);
+          release(prev);
         }
         prev = stage;
         if (++stage == STAGES) {
@@ -214,9 +249,14 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       wgmma_wait<0>();
       wgmma_fence_operand(acc);
-      mbar_arrive(&empty[prev]);
+      release(prev);
       epi.tile(c, acc);
     }
+  }
+  // The peer may still multicast into this CTA's ring or arrive on its barriers until it is done too.
+  if (CLUSTER > 1) {
+    __syncwarp();
+    cluster_sync_all();
   }
 }
 

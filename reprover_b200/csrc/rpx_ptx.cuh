@@ -169,13 +169,16 @@ RPX_DEVICE void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// Arrive on the barrier at `bar`'s offset in the shared memory of cluster CTA `cta`.
+// Arrive on the barrier at `bar`'s offset in the shared memory of cluster CTA `cta`.  The arrive has the default
+// CTA-scope release semantics: the pipelines use it to hand a stage back once their wgmma reads of it have
+// completed (wgmma.wait_group), which needs no ordering of other memory operations.  `.release.cluster` would
+// compile to a GPU-scope MEMBAR before every arrival, which waits for the thread's outstanding global stores.
 RPX_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n"
       ".reg .b32 ra;\n"
       "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
       "}\n" ::"r"(smem_u32(bar)),
       "r"(cta)
       : "memory");
