@@ -269,6 +269,25 @@ int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const
                            float* d_h32, void* d_h16, float* d_ss_out, const void* d_prefetch,
                            size_t prefetch_bytes, void* stream);
 
+/* The relative-position bias table of the attention kernel, built as rpx_encoder_create builds it:
+ * d_lut [n_heads][2 R + 1] fp32 (R = rel_max_distance), lut[h][delta + R] = d_rel_bias[bucket(delta)][h] for
+ * delta = key - query, from an HF-layout relative_attention_bias table d_rel_bias [rel_buckets][n_heads] fp32.
+ * Rejects the configs rpx_encoder_create rejects.  Synchronises `stream`; stages the (2 R + 1)-entry bucket
+ * table in a stream-ordered allocation it frees before returning. */
+int rpx_debug_attention_lut(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets,
+                            int32_t rel_max_distance, float* d_lut, void* stream);
+/* The encoder's attention, launched as the forward pass launches it for n_tokens tokens on the throughput
+ * (latency = 0) or latency path, PDL scope set as forward() sets it.
+ *   d_qkv   [n_tokens, 3 * n_heads * 64] bf16: q | k | v, head h in columns [64 h, 64 h + 64) of each
+ *   d_out   [n_tokens, n_heads * 64] bf16; rows of tokens outside every sequence are not written
+ *   d_cu_seqlens  [n_seqs + 1] int32 token offsets of the packed sequences on the device; the caller
+ *           guarantees 0 = cu[0] < cu[1] < ... < cu[n_seqs] <= n_tokens and max_len >= every length
+ *   d_lut   from rpx_debug_attention_lut with the same n_heads and rel_max_distance
+ * 1 <= n_seqs <= 65535 (the grid limit; more returns RPX_ERR_UNSUPPORTED).  Does not synchronise. */
+int rpx_debug_attention(int32_t latency, const void* d_qkv, void* d_out, const int32_t* d_cu_seqlens,
+                        const float* d_lut, int32_t n_tokens, int32_t n_seqs, int32_t max_len,
+                        int32_t n_heads, int32_t rel_max_distance, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

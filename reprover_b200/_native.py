@@ -118,6 +118,9 @@ _SIGNATURES = {
     "rpx_debug_encoder_gemm": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "rpx_debug_attention_lut": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "rpx_debug_attention": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
 }
 
 RPX_EGEMM_QKV = 0

@@ -51,6 +51,7 @@ struct ProfRec {
 
 // T5 relative-position bucket, bidirectional (HF modeling_t5.py:189-234), float32 math
 // like the reference implementation.  Host function, exported for the CPU parity test.
+// Precondition (check_rel_attention): max_distance > num_buckets / 4, else the log-spaced branch divides by 0.
 extern "C" int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num_buckets, int32_t max_distance) {
   int nb = num_buckets / 2;
   int ret = relative_position > 0 ? nb : 0;
@@ -123,17 +124,22 @@ PackedLayout packed_layout(const rpx_t5_config& c) {
   return L;
 }
 
+// The bucket formula takes log(max_distance / max_exact) with max_exact = buckets / 4, so max_distance must
+// exceed it; 2048 bounds the bias table the attention kernel keeps in shared memory.
+int check_rel_attention(int rel_buckets, int rel_max_distance) {
+  RPX_REQUIRE(rel_buckets >= 4 && rel_buckets % 4 == 0 && rel_max_distance > rel_buckets / 4 && rel_max_distance <= 2048,
+              RPX_ERR_UNSUPPORTED, "unsupported relative attention config (%d buckets, max distance %d)", rel_buckets,
+              rel_max_distance);
+  return RPX_OK;
+}
+
 int validate_cfg(const rpx_t5_config* c) {
   RPX_REQUIRE(c != nullptr, RPX_ERR_INVALID, "config is null");
   RPX_REQUIRE(c->d_kv == 64, RPX_ERR_UNSUPPORTED, "d_kv=%d: only 64 is implemented", c->d_kv);
   RPX_REQUIRE(c->d_model % 64 == 0 && c->d_model > 0, RPX_ERR_UNSUPPORTED, "d_model=%d must be a multiple of 64", c->d_model);
   RPX_REQUIRE(c->d_ff % 128 == 0 && c->d_ff > 0, RPX_ERR_UNSUPPORTED, "d_ff=%d must be a multiple of 128", c->d_ff);
   RPX_REQUIRE(c->num_heads > 0 && c->num_layers > 0 && c->vocab_size > 0, RPX_ERR_INVALID, "bad config");
-  RPX_REQUIRE(c->rel_buckets >= 4 && c->rel_buckets % 4 == 0 && c->rel_max_distance >= c->rel_buckets / 4 &&
-                  c->rel_max_distance <= 2048,
-              RPX_ERR_UNSUPPORTED, "unsupported relative attention config (%d buckets, max distance %d)",
-              c->rel_buckets, c->rel_max_distance);
-  return RPX_OK;
+  return check_rel_attention(c->rel_buckets, c->rel_max_distance);
 }
 
 __global__ void bias_lut_kernel(const float* __restrict__ rel_bias, const int32_t* __restrict__ buckets,
@@ -142,6 +148,21 @@ __global__ void bias_lut_kernel(const float* __restrict__ rel_bias, const int32_
   if (i >= n_heads * width) return;
   const int h = i / width, j = i % width;
   lut[i] = rel_bias[buckets[j] * n_heads + h];
+}
+
+// Relative-position bias LUT: lut[h][delta + R] = rel_bias[bucket(delta)][h] for delta = key - query in [-R, R].
+// The bucket table is computed on the host and staged through `d_buckets` (2R + 1 int32).  Synchronises `st`:
+// the host table is pageable and dies on return.  The caller has checked the config (check_rel_attention).
+int build_bias_lut(const float* d_rel_bias, int n_heads, int rel_buckets, int R, int32_t* d_buckets, float* d_lut,
+                   cudaStream_t st) {
+  const int width = 2 * R + 1;
+  std::vector<int32_t> buckets(width);
+  for (int j = 0; j < width; ++j) buckets[j] = rpx_t5_relative_bucket(j - R, rel_buckets, R);
+  RPX_CUDA_OK(cudaMemcpyAsync(d_buckets, buckets.data(), (size_t)width * 4, cudaMemcpyHostToDevice, st));
+  bias_lut_kernel<<<ceil_div(n_heads * width, 256), 256, 0, st>>>(d_rel_bias, d_buckets, d_lut, n_heads, width);
+  RPX_CUDA_OK(cudaGetLastError());
+  RPX_CUDA_OK(cudaStreamSynchronize(st));
+  return RPX_OK;
 }
 
 struct Workspace {
@@ -469,15 +490,8 @@ int rpx_encoder_create(const rpx_t5_config* cfg, const rpx_t5_weights* w, void* 
   e->emb = reinterpret_cast<const float*>(base + L.emb);
   e->final_ln = reinterpret_cast<const float*>(base + L.final_ln);
 
-  // relative-position bias LUT: lut[h][delta + R] = rel_bias[bucket(delta)][h]
-  const int R = cfg->rel_max_distance, width = 2 * R + 1;
-  std::vector<int32_t> buckets(width);
-  for (int j = 0; j < width; ++j) buckets[j] = rpx_t5_relative_bucket(j - R, cfg->rel_buckets, R);
-  CUDA_E(cudaMemcpyAsync(base + L.bucket_tmp, buckets.data(), (size_t)width * 4, cudaMemcpyHostToDevice, st));
-  bias_lut_kernel<<<ceil_div(cfg->num_heads * width, 256), 256, 0, st>>>(
-      w->d_rel_bias, reinterpret_cast<const int32_t*>(base + L.bucket_tmp), reinterpret_cast<float*>(base + L.bias_lut),
-      cfg->num_heads, width);
-  CUDA_E(cudaGetLastError());
+  TRY_E(build_bias_lut(w->d_rel_bias, cfg->num_heads, cfg->rel_buckets, cfg->rel_max_distance,
+                       reinterpret_cast<int32_t*>(base + L.bucket_tmp), reinterpret_cast<float*>(base + L.bias_lut), st));
   e->bias_lut = reinterpret_cast<const float*>(base + L.bias_lut);
 
   e->layers.resize(cfg->num_layers);
@@ -499,7 +513,7 @@ int rpx_encoder_create(const rpx_t5_config* cfg, const rpx_t5_weights* w, void* 
     e->layers[l] = LayerW{qkv, o, wi, wo};
     e->layer_bytes = L.layer_stride;
   }
-  // `buckets` is pageable host memory: make sure the H2D staging has finished before it dies.
+  // the packed image is complete on return, so the caller may release the fp32 weights at once
   CUDA_E(cudaStreamSynchronize(st));
 #undef TRY_E
 #undef CUDA_E
@@ -648,6 +662,35 @@ int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const
     case RPX_EGEMM_FFN_UP: return ffn_up_gemm(lat, T, d_A, d_B, N, K, rs, out, st);
     default: return ffn_down_gemm(lat, T, d_A, d_B, N, K, d_h32, h16, d_ss_out, st);
   }
+}
+
+int rpx_debug_attention_lut(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets, int32_t rel_max_distance,
+                            float* d_lut, void* stream) {
+  RPX_REQUIRE(d_rel_bias && d_lut, RPX_ERR_INVALID, "rpx_debug_attention_lut: null argument");
+  RPX_REQUIRE(n_heads > 0, RPX_ERR_INVALID, "rpx_debug_attention_lut: n_heads=%d", n_heads);
+  RPX_TRY(check_rel_attention(rel_buckets, rel_max_distance));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  int32_t* d_buckets = nullptr;
+  RPX_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d_buckets), (size_t)(2 * rel_max_distance + 1) * 4, st));
+  const int rc = build_bias_lut(d_rel_bias, n_heads, rel_buckets, rel_max_distance, d_buckets, d_lut, st);
+  RPX_CUDA_OK(cudaFreeAsync(d_buckets, st));
+  return rc;
+}
+
+int rpx_debug_attention(int32_t latency, const void* d_qkv, void* d_out, const int32_t* d_cu_seqlens,
+                        const float* d_lut, int32_t n_tokens, int32_t n_seqs, int32_t max_len, int32_t n_heads,
+                        int32_t rel_max_distance, void* stream) {
+  RPX_REQUIRE(d_qkv && d_out && d_cu_seqlens && d_lut, RPX_ERR_INVALID, "rpx_debug_attention: null argument");
+  RPX_REQUIRE(n_tokens > 0 && max_len > 0 && n_heads > 0, RPX_ERR_INVALID,
+              "rpx_debug_attention: n_tokens=%d max_len=%d n_heads=%d", n_tokens, max_len, n_heads);
+  RPX_REQUIRE(n_seqs > 0, RPX_ERR_INVALID, "rpx_debug_attention: n_seqs=%d", n_seqs);
+  RPX_REQUIRE(n_seqs <= 65535, RPX_ERR_UNSUPPORTED, "rpx_debug_attention: n_seqs=%d exceeds the 65535 grid limit", n_seqs);
+  RPX_REQUIRE(rel_max_distance > 0 && rel_max_distance <= 2048, RPX_ERR_INVALID,
+              "rpx_debug_attention: rel_max_distance=%d", rel_max_distance);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PdlScope pdl_scope(latency != 0 || n_tokens <= kPdlMaxTokens);
+  return launch_t5_attention(static_cast<const __nv_bfloat16*>(d_qkv), static_cast<__nv_bfloat16*>(d_out), d_cu_seqlens,
+                             d_lut, n_tokens, n_seqs, max_len, n_heads, 64, rel_max_distance, st);
 }
 
 int rpx_encoder_read_profile(rpx_encoder* enc, float* h_ms, int64_t* h_launches) {

@@ -109,6 +109,51 @@ def test_encoder_gemm_entry_rejects_bad_input_before_touching_a_device(rpx_lib):
     assert rc == _native.RPX_ERR_UNSUPPORTED and "multiple of 256" in _native.last_error()
 
 
+def test_relative_attention_config_bound(rpx_lib):
+    """max_distance must exceed buckets / 4: at equality the bucket formula divides by log(1) = 0 (for (32, 8)
+    rpx_t5_relative_bucket would return a huge negative bucket and the LUT kernel would read far out of bounds)."""
+    def cfg(buckets, R):
+        return _native.T5Config(vocab_size=384, d_model=1472, d_kv=64, d_ff=3584, num_layers=12, num_heads=6,
+                                rel_buckets=buckets, rel_max_distance=R, ln_eps=1e-6)
+
+    for buckets, R in ((32, 8), (8, 2)):
+        assert rpx_lib.rpx_encoder_packed_bytes(C.byref(cfg(buckets, R))) == 0
+        assert "relative attention config" in _native.last_error()
+    for buckets, R in ((32, 9), (32, 128), (64, 2048)):
+        assert rpx_lib.rpx_encoder_packed_bytes(C.byref(cfg(buckets, R))) > 0, (buckets, R)
+
+
+def test_attention_entry_points_match_header(rpx_lib):
+    """The two attention test entry points take as many arguments in the ctypes table as in include/rpx.h."""
+    text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "rpx.h").read_text(), flags=re.S)
+    for name in ("rpx_debug_attention_lut", "rpx_debug_attention"):
+        params = re.search(rf"\b{name}\s*\(([^)]*)\)", text).group(1)
+        assert len(params.split(",")) == len(_native._SIGNATURES[name][1]), name
+        assert hasattr(rpx_lib, name)
+
+
+@needs_no_gpu
+def test_attention_entry_points_reject_bad_input_before_touching_a_device(rpx_lib):
+    buf = (C.c_uint8 * 1024)()
+    att = rpx_lib.rpx_debug_attention
+    assert att(0, None, buf, buf, buf, 4, 1, 4, 1, 128, None) == _native.RPX_ERR_INVALID
+    assert att(0, buf, buf, None, buf, 4, 1, 4, 1, 128, None) == _native.RPX_ERR_INVALID
+    assert att(0, buf, buf, buf, buf, 0, 1, 4, 1, 128, None) == _native.RPX_ERR_INVALID
+    assert att(0, buf, buf, buf, buf, 4, 1, 0, 1, 128, None) == _native.RPX_ERR_INVALID
+    assert att(0, buf, buf, buf, buf, 4, 1, 4, 0, 128, None) == _native.RPX_ERR_INVALID
+    assert att(0, buf, buf, buf, buf, 4, 0, 4, 1, 128, None) == _native.RPX_ERR_INVALID
+    rc = att(0, buf, buf, buf, buf, 4, 65536, 4, 1, 128, None)
+    assert rc == _native.RPX_ERR_UNSUPPORTED and "65535" in _native.last_error()
+    lut = rpx_lib.rpx_debug_attention_lut
+    assert lut(None, 6, 32, 128, buf, None) == _native.RPX_ERR_INVALID
+    assert lut(buf, 0, 32, 128, buf, None) == _native.RPX_ERR_INVALID
+    assert lut(buf, 6, 32, 8, buf, None) == _native.RPX_ERR_UNSUPPORTED
+    assert "relative attention config" in _native.last_error()
+    # valid arguments reach the device, and there is none
+    assert lut(buf, 6, 32, 128, buf, None) == _native.RPX_ERR_CUDA and _native.last_error()
+    assert att(1, buf, buf, buf, buf, 4, 1, 4, 1, 128, None) == _native.RPX_ERR_CUDA and _native.last_error()
+
+
 @needs_no_gpu
 def test_python_product_path_refuses_cpu():
     from reprover_b200.engine import T5EncoderEngine

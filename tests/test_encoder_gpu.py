@@ -204,7 +204,7 @@ def test_latency_path_batch_equals_single(rpx_lib, cuda_device):
         alone = eng.encode_bytes(np.frombuffer(sbytes, dtype=np.uint8), np.array([0, len(sbytes)], dtype=np.int64), 2048,
                                  out_dtype=torch.float32)
         assert torch.equal(alone[0], together[i]), (i, len(sbytes))
-    # sequences that take one, two and three 256-key attention blocks in the same call
+    # sequences of 40, 300 and 620 tokens (1, 5 and 10 of the kernel's 64-key steps) in the same call
     parts = [synth.split_strings(*synth.synth_states(1, seed=40 + i, min_len=n, max_len=n))[0] for i, n in enumerate((40, 300, 620))]
     offs = np.concatenate([[0], np.cumsum([len(p) for p in parts])]).astype(np.int64)
     mixed = eng.encode_bytes(np.frombuffer(b"".join(parts), dtype=np.uint8), offs, 2048, out_dtype=torch.float32)
