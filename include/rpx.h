@@ -130,6 +130,26 @@ int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* 
                    int32_t batch, int32_t seq_len, void* d_out, int32_t out_dtype,
                    void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* The encoder's per-token output, `last_hidden_state` of HF `T5EncoderModel` (the final RMSNorm of every
+ * token, modeling_t5.py:782), for callers that pool it themselves.  Replaces
+ *   self.encoder(input_ids=..., attention_mask=..., return_dict=True).last_hidden_state   retrieval/model.py:101-105
+ *   self.encoder(input_ids, attention_mask)[0]                                            retrieval/model.py:97-99
+ * and the README's `model(tokenized_s.input_ids).last_hidden_state` (no mask).
+ *   d_attention_mask  int64 [batch, seq_len], or NULL: HF's attention_mask=None, every position is a token
+ *                     (pad id 0 included) and every row is seq_len long
+ *   d_out             [batch, seq_len, d_model], RPX_DTYPE_BF16 or RPX_DTYPE_F32, 16-byte aligned; row (b, p)
+ *                     is token p of sequence b.  Nothing past batch * seq_len rows is written.
+ * Validation, workspace rule (rpx_encoder_workspace_bytes(enc, batch * seq_len, batch)), the id-range check
+ * and the synchronisation are those of rpx_encode_ids; a non-NULL mask must be a right-padded prefix mask
+ * (RPX_ERR_MASK otherwise).  Without a mask the length readback is skipped, but the call still synchronises
+ * once to check the ids.  The one deliberate difference from HF: positions past a row's mask length are
+ * written as zeros, where HF computes values for them (the pad queries attend to the real keys).  No code of the
+ * reference reads them: `_encode` and the README both multiply the hidden states by the mask before pooling. */
+int rpx_encode_ids_hidden(rpx_encoder* enc, const int64_t* d_input_ids,
+                          const int64_t* d_attention_mask /* NULL: every position is a token */,
+                          int32_t batch, int32_t seq_len, void* d_out /* [batch, seq_len, d_model] */,
+                          int32_t out_dtype, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* Latency path: encode calls with at most `max_tokens` packed tokens (0 = never, the default) run on
  * kernels shaped for ONE proof state — the reference's per-state call (`retrieve`,
  * retrieval/model.py:348-357) — instead of the 128 x 128 tiles that are sized for re-indexing: narrow

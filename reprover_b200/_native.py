@@ -86,6 +86,8 @@ _SIGNATURES = {
                                    C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_encode_ids": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "rpx_encode_ids_hidden": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                        C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_encoder_set_latency_tokens": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_t5_relative_bucket": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
     "rpx_encoder_set_debug_hidden": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -1,6 +1,7 @@
 // rpx_elementwise.cu — the HBM-bound byte / row kernels around the GEMMs:
 // ByT5 tokenisation (K1 prologue), embedding gather (K1), final RMSNorm + masked
-// mean-pool + L2 normalise (K2 + K10), attention-mask validation, weight packing.
+// mean-pool + L2 normalise (K2 + K10) or final RMSNorm per token (the hidden-state output),
+// attention-mask validation, weight packing.
 // All are coalesced, vectorised (16-byte) row streams; none is reshaped into a GEMM.
 #include "rpx_common.cuh"
 #include "rpx_kernels.cuh"
@@ -318,6 +319,66 @@ pool_final_kernel(const float* __restrict__ scratch, const float* __restrict__ l
   }
 }
 
+// Final RMSNorm of every token into a padded [batch, seq_len, d_model] output (HF T5Stack's
+// `final_layer_norm`, modeling_t5.py:782, i.e. `last_hidden_state`).  One warp per output row (b, p), lanes
+// across the columns, 8 columns per lane and trip (two 16-byte loads of h32 and of the weight, one 16-byte store
+// of bf16 or two of fp32).  Row (b, p) holds token cu[b] + p while p < len_b and zeros past it.  The row scale
+// sums the ss parts in the order of the pool kernel the forward pass would run: part after part as in
+// pool_normalize_kernel, or (`lane_ss`, the latency path) lane-strided and reduced by shuffles as in
+// pool_partial_kernel; then the same rsqrtf.
+__global__ void hidden_store_kernel(const float* __restrict__ h32, const float* __restrict__ ss, int ss_stride,
+                                    int n_parts, bool lane_ss, const float* __restrict__ ln_w,
+                                    const int32_t* __restrict__ cu_tokens, void* __restrict__ out, int out_dtype,
+                                    int64_t n_rows, int seq_len, int d_model, float eps) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= n_rows) return;
+  const int b = (int)(row / seq_len), p = (int)(row % seq_len);
+  const int t0 = cu_tokens[b], len = cu_tokens[b + 1] - t0;
+  const int n8 = d_model >> 3;
+  float4* o32 = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + row * d_model);
+  uint4* o16 = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(out) + row * d_model);
+  if (p >= len) {
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int c = lane; c < n8; c += 32) {
+      if (out_dtype == RPX_DTYPE_F32) {
+        o32[2 * c] = z;
+        o32[2 * c + 1] = z;
+      } else {
+        o16[c] = make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+    return;
+  }
+  const int t = t0 + p;
+  float sum = 0.f;
+  if (lane_ss) {
+    for (int q = lane; q < n_parts; q += 32) sum += ss[(int64_t)q * ss_stride + t];
+#pragma unroll
+    for (int off = 16; off; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
+  } else {
+    for (int q = 0; q < n_parts; ++q) sum += ss[(int64_t)q * ss_stride + t];
+  }
+  const float rs = rsqrtf(sum * (1.0f / (float)d_model) + eps);
+  const float4* src = reinterpret_cast<const float4*>(h32 + (int64_t)t * d_model);
+  const float4* w4 = reinterpret_cast<const float4*>(ln_w);
+  for (int c = lane; c < n8; c += 32) {
+    const float4 a = src[2 * c], bb = src[2 * c + 1];
+    const float4 wa = w4[2 * c], wb = w4[2 * c + 1];
+    const float4 ya = make_float4(a.x * rs * wa.x, a.y * rs * wa.y, a.z * rs * wa.z, a.w * rs * wa.w);
+    const float4 yb = make_float4(bb.x * rs * wb.x, bb.y * rs * wb.y, bb.z * rs * wb.z, bb.w * rs * wb.w);
+    if (out_dtype == RPX_DTYPE_F32) {
+      o32[2 * c] = ya;
+      o32[2 * c + 1] = yb;
+    } else {
+      o16[c] = make_uint4(pack_bf16x2(ya.x, ya.y), pack_bf16x2(ya.z, ya.w), pack_bf16x2(yb.x, yb.y),
+                          pack_bf16x2(yb.z, yb.w));
+    }
+  }
+}
+
 __global__ void pack_weight_kernel(const float* __restrict__ src, const float* __restrict__ scale,
                                    __nv_bfloat16* __restrict__ dst, int n_rows, int n_cols, int dst_row0,
                                    int blk, int blk_stride) {
@@ -384,6 +445,17 @@ int launch_pool_normalize(const float* h32, const float* ss, int ss_stride, int 
   }
   RPX_CUDA_OK(launch_pdl(pool_normalize_kernel, dim3(n_seqs), dim3(threads), 0, stream, pdl_enabled(), h32, ss, ss_stride,
                          n_parts, ln_w, cu_tokens, out, out_dtype, d_model, eps));
+  return RPX_OK;
+}
+
+int launch_hidden_store(const float* h32, const float* ss, int ss_stride, int n_parts, bool lane_ss, const float* ln_w,
+                        const int32_t* cu_tokens, void* out, int out_dtype, int batch, int seq_len, int d_model,
+                        float eps, cudaStream_t stream) {
+  RPX_REQUIRE(d_model % 8 == 0, RPX_ERR_UNSUPPORTED, "hidden store: d_model=%d must be a multiple of 8", d_model);
+  RPX_REQUIRE(out_dtype == RPX_DTYPE_BF16 || out_dtype == RPX_DTYPE_F32, RPX_ERR_INVALID, "hidden store: bad out dtype");
+  const int64_t n_rows = (int64_t)batch * seq_len;
+  RPX_CUDA_OK(launch_pdl(hidden_store_kernel, dim3((unsigned)ceil_div64(n_rows, 8)), dim3(256), 0, stream, pdl_enabled(), h32,
+                         ss, ss_stride, n_parts, lane_ss, ln_w, cu_tokens, out, out_dtype, n_rows, seq_len, d_model, eps));
   return RPX_OK;
 }
 

@@ -371,9 +371,15 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   return RPX_OK;
 }
 
-// The forward pass proper.  ws.ids / ws.cu_tokens are already populated on `st`.
-int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void* d_out, int out_dtype,
-            cudaStream_t st) {
+// What forward() writes after the last block.
+//   kPooled  final RMSNorm + masked mean + L2 normalise: [S, D]
+//   kHidden  final RMSNorm of every token (`last_hidden_state`): [S, seq_len, D], rows past a sequence's length zeroed
+enum class OutKind { kPooled, kHidden };
+
+// The forward pass proper.  ws.ids / ws.cu_tokens are already populated on `st`.  `seq_len` is the padded row
+// length of a kHidden output (unused for kPooled).
+int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutKind kind, int seq_len, void* d_out,
+            int out_dtype, cudaStream_t st) {
   const rpx_t5_config& c = e->cfg;
   const int D = c.d_model, inner = e->inner, F = c.d_ff;
   // the latency path needs d_ff in 128-unit blocks for its split-B tiles (validate_cfg) and narrow-tile n
@@ -425,7 +431,12 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, void
     }
     RPX_TRY(dump(l + 1));
   }
-  {
+  if (kind == OutKind::kHidden) {
+    Prof p(e, st, 6);
+    // the latency path pools with pool_partial_kernel: its order of the ss parts keeps the rows consistent with it
+    RPX_TRY(launch_hidden_store(ws.h32, ws.ssA, T, P, latency, e->final_ln, ws.cu_tokens, d_out, out_dtype, S, seq_len, D,
+                                c.ln_eps, st));
+  } else {
     Prof p(e, st, 6);
     // latency path: per-group partial rows go where the (now dead) FFN activations were — T rows of d_ff
     // bf16 hold T rows of d_model fp32 when d_ff >= 2 d_model (else the single-kernel pool runs)
@@ -568,16 +579,22 @@ int rpx_encode_bytes(rpx_encoder* enc, const uint8_t* d_bytes, const int64_t* h_
   RPX_CUDA_OK(cudaMemcpyAsync(ws.cu_tokens, cu.data(), ((size_t)n_seqs + 1) * 4, cudaMemcpyHostToDevice, st));
   RPX_CUDA_OK(cudaMemcpyAsync(ws.cu_bytes, h_offsets, ((size_t)n_seqs + 1) * 8, cudaMemcpyHostToDevice, st));
   RPX_TRY(launch_tokenize_bytes(d_bytes, ws.cu_bytes, ws.cu_tokens, ws.ids, n_seqs, T, st));
-  return forward(enc, ws, T, n_seqs, max_len, d_out, out_dtype, st);
+  return forward(enc, ws, T, n_seqs, max_len, OutKind::kPooled, 0, d_out, out_dtype, st);
 }
 
-int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* d_attention_mask, int32_t batch,
-                   int32_t seq_len, void* d_out, int32_t out_dtype, void* d_workspace, size_t workspace_bytes,
-                   void* stream) {
-  RPX_REQUIRE(enc && d_input_ids && d_attention_mask && d_out && d_workspace, RPX_ERR_INVALID,
-              "rpx_encode_ids: null argument");
-  RPX_REQUIRE(batch > 0 && seq_len > 0, RPX_ERR_INVALID, "rpx_encode_ids: batch=%d seq_len=%d", batch, seq_len);
-  RPX_REQUIRE((int64_t)batch * seq_len < (int64_t)INT32_MAX, RPX_ERR_UNSUPPORTED, "rpx_encode_ids: batch too large");
+}  // extern "C"
+
+namespace {
+
+// rpx_encode_ids and rpx_encode_ids_hidden on padded int64 [batch, seq_len] ids: validate, take the row lengths
+// from the mask (seq_len for every row without one), pack the ids, run the forward pass, report ids outside the
+// vocabulary.  `fn` names the entry point in error messages.
+int encode_padded_ids(const char* fn, rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* d_attention_mask,
+                      int32_t batch, int32_t seq_len, OutKind kind, void* d_out, int32_t out_dtype, void* d_workspace,
+                      size_t workspace_bytes, void* stream) {
+  RPX_REQUIRE(enc && d_input_ids && d_out && d_workspace, RPX_ERR_INVALID, "%s: null argument", fn);
+  RPX_REQUIRE(batch > 0 && seq_len > 0, RPX_ERR_INVALID, "%s: batch=%d seq_len=%d", fn, batch, seq_len);
+  RPX_REQUIRE((int64_t)batch * seq_len < (int64_t)INT32_MAX, RPX_ERR_UNSUPPORTED, "%s: batch too large", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // Worst case all tokens valid: the workspace must fit that (callers size it with batch*seq_len).
   const Workspace ws_max = carve(enc, static_cast<uint8_t*>(d_workspace), (int64_t)batch * seq_len, batch);
@@ -585,14 +602,16 @@ int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* 
               workspace_bytes);
   RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
   RPX_CUDA_OK(cudaMemsetAsync(ws_max.flag, 0, 4, st));
-  RPX_TRY(launch_mask_lengths(d_attention_mask, ws_max.lens, ws_max.flag, batch, seq_len, st));
   auto& lens = enc->h_lens;
-  lens.resize((size_t)batch + 1);
-  RPX_CUDA_OK(cudaMemcpyAsync(lens.data(), ws_max.lens, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(&lens[batch], ws_max.flag, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaStreamSynchronize(st));
-  RPX_REQUIRE(lens[batch] == 0, RPX_ERR_MASK,
-              "attention_mask must be a right-padded prefix of ones with at least one token per row");
+  lens.assign((size_t)batch + 1, seq_len);
+  if (d_attention_mask) {
+    RPX_TRY(launch_mask_lengths(d_attention_mask, ws_max.lens, ws_max.flag, batch, seq_len, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(lens.data(), ws_max.lens, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(&lens[batch], ws_max.flag, 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaStreamSynchronize(st));
+    RPX_REQUIRE(lens[batch] == 0, RPX_ERR_MASK,
+                "attention_mask must be a right-padded prefix of ones with at least one token per row");
+  }
   auto& cu = enc->h_cu_tokens;
   cu.resize((size_t)batch + 1);
   cu[0] = 0;
@@ -607,13 +626,36 @@ int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* 
   const Workspace ws = carve(enc, static_cast<uint8_t*>(d_workspace), T, batch);
   RPX_CUDA_OK(cudaMemcpyAsync(ws.cu_tokens, cu.data(), ((size_t)batch + 1) * 4, cudaMemcpyHostToDevice, st));
   RPX_TRY(launch_pack_ids(d_input_ids, ws.cu_tokens, ws.ids, batch, seq_len, T, enc->cfg.vocab_size, ws.flag, st));
-  RPX_TRY(forward(enc, ws, T, batch, max_len, d_out, out_dtype, st));
+  RPX_TRY(forward(enc, ws, T, batch, max_len, kind, seq_len, d_out, out_dtype, st));
   // ids outside [0, vocab) are reported after the fact (the forward ran with id 0 in their place).
   int32_t flag = 0;
   RPX_CUDA_OK(cudaMemcpyAsync(&flag, ws.flag, 4, cudaMemcpyDeviceToHost, st));
   RPX_CUDA_OK(cudaStreamSynchronize(st));
   RPX_REQUIRE((flag & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", enc->cfg.vocab_size);
   return RPX_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int rpx_encode_ids(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* d_attention_mask, int32_t batch,
+                   int32_t seq_len, void* d_out, int32_t out_dtype, void* d_workspace, size_t workspace_bytes,
+                   void* stream) {
+  RPX_REQUIRE(d_attention_mask, RPX_ERR_INVALID, "rpx_encode_ids: null argument");
+  return encode_padded_ids("rpx_encode_ids", enc, d_input_ids, d_attention_mask, batch, seq_len, OutKind::kPooled, d_out,
+                           out_dtype, d_workspace, workspace_bytes, stream);
+}
+
+int rpx_encode_ids_hidden(rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* d_attention_mask, int32_t batch,
+                          int32_t seq_len, void* d_out, int32_t out_dtype, void* d_workspace, size_t workspace_bytes,
+                          void* stream) {
+  RPX_REQUIRE(out_dtype == RPX_DTYPE_BF16 || out_dtype == RPX_DTYPE_F32, RPX_ERR_INVALID,
+              "rpx_encode_ids_hidden: out_dtype=%d", out_dtype);
+  RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_out) & 15) == 0, RPX_ERR_INVALID,
+              "rpx_encode_ids_hidden: d_out must be 16-byte aligned");
+  return encode_padded_ids("rpx_encode_ids_hidden", enc, d_input_ids, d_attention_mask, batch, seq_len, OutKind::kHidden,
+                           d_out, out_dtype, d_workspace, workspace_bytes, stream);
 }
 
 int rpx_encoder_set_latency_tokens(rpx_encoder* enc, int32_t max_tokens) {

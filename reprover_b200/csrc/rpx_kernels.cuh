@@ -33,6 +33,13 @@ int launch_embed(const int32_t* ids, const float* table, float* h32, __nv_bfloat
 int launch_pool_normalize(const float* h32, const float* ss, int ss_stride, int n_parts, const float* ln_w,
                           const int32_t* cu_tokens, void* out, int out_dtype, int n_seqs, int d_model,
                           float eps, cudaStream_t stream, float* group_scratch = nullptr, int max_len = 0);
+// Final RMSNorm of every token (the encoder's `last_hidden_state`) into a padded [batch, seq_len, d_model] output:
+//   out[b, p] = w .* h32[cu[b] + p] * rs[cu[b] + p]  for p < len_b,  0  for p >= len_b.
+// `lane_ss`: sum the ss parts in pool_partial_kernel's order (latency path) instead of pool_normalize_kernel's.
+// `out` must be 16-byte aligned.
+int launch_hidden_store(const float* h32, const float* ss, int ss_stride, int n_parts, bool lane_ss, const float* ln_w,
+                        const int32_t* cu_tokens, void* out, int out_dtype, int batch, int seq_len, int d_model,
+                        float eps, cudaStream_t stream);
 
 // Weight packing (rpx_encoder_create): dst[n, k] = bf16(src[n, k] * scale[k]) (scale may be null),
 // rows written at dst_row0 + (n / blk) * blk_stride + (n % blk)  (FFN interleave when blk_stride != blk).

@@ -10,7 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import json
 import os
-from typing import Dict, Iterable, List, Optional, Sequence, Tuple, Union
+from typing import Dict, Iterable, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -89,8 +89,29 @@ def _stream_ptr(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
 
 
+class EncoderConfig(dict):
+    """The checkpoint's config.json as a dict that also answers attribute access the way an HF `T5Config`
+    does (`encoder.config.hidden_size`, retrieval/model.py:90; `hidden_size` is HF's alias of `d_model`)."""
+
+    _ALIASES = {"hidden_size": "d_model"}
+
+    def __getattr__(self, name: str):
+        try:
+            return self[self._ALIASES.get(name, name)]
+        except KeyError:
+            raise AttributeError(name) from None
+
+
+class EncoderOutput(NamedTuple):
+    """What HF `T5EncoderModel` returns, as far as the reference reads it: `.last_hidden_state`
+    (retrieval/model.py:101-105) or `[0]` (:97-99)."""
+
+    last_hidden_state: torch.Tensor
+
+
 class T5EncoderEngine:
-    """ByT5/T5 encoder + mean-pool + L2-normalise on one GPU (`rpx_encode_*`)."""
+    """ByT5/T5 encoder + mean-pool + L2-normalise on one GPU (`rpx_encode_*`); called like HF's
+    `T5EncoderModel`, it returns the per-token hidden states instead (`rpx_encode_ids_hidden`)."""
 
     def __init__(self, config: Dict, state_dict: Dict[str, torch.Tensor], device: Union[int, str, torch.device],
                  max_tokens_per_call: int = 1 << 18) -> None:
@@ -99,7 +120,7 @@ class T5EncoderEngine:
         if self.device.type != "cuda":
             raise RuntimeError(
                 f"T5EncoderEngine needs a CUDA device (got {self.device}); this engine has no CPU path")
-        self.config = dict(config)
+        self.config = EncoderConfig(config)
         missing = [k for k in required_weight_keys(config) if k not in state_dict]
         if "shared.weight" not in state_dict and "encoder.embed_tokens.weight" not in state_dict:
             missing.insert(0, "shared.weight (or encoder.embed_tokens.weight)")
@@ -290,6 +311,41 @@ class T5EncoderEngine:
                                                   self._out_dtype(out_dtype), ws.data_ptr(), ws.numel(),
                                                   _stream_ptr(self.device)))
         return out
+
+    @property
+    def dtype(self) -> torch.dtype:
+        """The compute dtype, read by the reference as `self.encoder.dtype` (retrieval/model.py:190-195): bf16,
+        what the reference's model is on this GPU after `load_hf`."""
+        return torch.bfloat16
+
+    def __call__(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None, return_dict: bool = True,
+                 out_dtype: torch.dtype = torch.bfloat16, *, head_mask=None, inputs_embeds=None,
+                 output_attentions: Optional[bool] = None, output_hidden_states: Optional[bool] = None) -> EncoderOutput:
+        """HF `T5EncoderModel.forward` as the reference calls it (`rpx_encode_ids_hidden`):
+        `.last_hidden_state` (or `[0]`) is [B, L, d_model] on the engine's device.  `attention_mask=None`
+        treats every position as a token, as HF does.  With a mask, which must be a right-padded prefix mask,
+        positions past a row's length are zeros (HF computes values there that no reference code reads)."""
+        unsupported = {"head_mask": head_mask is not None, "inputs_embeds": inputs_embeds is not None,
+                       "output_attentions": bool(output_attentions), "output_hidden_states": bool(output_hidden_states)}
+        asked = [k for k, v in unsupported.items() if v]
+        if asked:
+            raise NotImplementedError(f"T5EncoderEngine returns the last hidden state only; not supported: {asked}")
+        if input_ids is None or input_ids.dim() != 2:
+            raise ValueError("input_ids must be a [batch, seq_len] tensor")
+        ids = input_ids.to(device=self.device, dtype=torch.int64).contiguous()
+        mask = None
+        if attention_mask is not None:
+            if attention_mask.shape != input_ids.shape:
+                raise ValueError(f"attention_mask {tuple(attention_mask.shape)} != input_ids {tuple(input_ids.shape)}")
+            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
+        B, L = ids.shape
+        out = torch.empty(B, L, self.hidden_size, dtype=out_dtype, device=self.device)
+        with torch.cuda.device(self.device):
+            ws = self._workspace(B * L, B)
+            _native.check(self.lib.rpx_encode_ids_hidden(
+                self._handle, ids.data_ptr(), None if mask is None else mask.data_ptr(), B, L, out.data_ptr(),
+                self._out_dtype(out_dtype), ws.data_ptr(), ws.numel(), _stream_ptr(self.device)))
+        return EncoderOutput(out)
 
     def set_latency_tokens(self, max_tokens: int) -> None:
         """Engine calls with at most `max_tokens` packed tokens take the latency path (narrow tiles: one
