@@ -254,6 +254,41 @@ int rpx_topk_merge_packed(const int64_t* d_packed, int32_t n_parts, int32_t nq, 
                           float* d_out_scores, double* d_out_scores64, int64_t* d_out_idx,
                           int32_t* d_out_count, void* stream);
 
+/* ------------------------------------------------------------------------------ BM25
+ * Replaces the scoring and ranking of the reference's BM25 baseline (retrieval/bm25/main.py:48-52):
+ *     scores = bm25.get_batch_scores(query_tokens, accessible);  np.argsort(scores)[::-1][:num_retrieved]
+ * with rank_bm25.BM25Okapi's arithmetic.  The index is an inverted index in CSR form, built on the host
+ * (reprover_b200/bm25.py) and owned by the caller:
+ *   d_term_ptr  [vocab + 1] int64  the postings of term t are [term_ptr[t], term_ptr[t + 1])
+ *   d_post_doc  [nnz] int32        document (premise) index, strictly ascending within a term
+ *   d_post_c    [nnz] fp64         the term's contribution to that document's score,
+ *                                  idf[t] * (tf * 2.5 / (tf + 1.5 * (0.25 + 0.75 * doc_len / avgdl)))
+ * A query is a list of term ids in query order, repeats included; an id outside [0, vocab) adds nothing, like a token
+ * the corpus does not contain.  A document's score is the fp64 sum ((0 + c(q1, d)) + c(q2, d)) + ... over the query
+ * tokens present in it, added in query order, so it equals get_batch_scores bit for bit.  Ranking: score descending,
+ * then index ascending (the reference's argsort leaves ties in no defined order).
+ */
+typedef struct rpx_bm25 rpx_bm25; /* opaque; the arrays must outlive it */
+int rpx_bm25_create(const int64_t* d_term_ptr, const int32_t* d_post_doc, const double* d_post_c, int32_t vocab,
+                    int64_t n_docs, int64_t nnz, rpx_bm25** out);
+int rpx_bm25_destroy(rpx_bm25* ix);
+/* 0 when the request is out of range (nq outside [1, 65535], k outside [1, 1024]). */
+size_t rpx_bm25_topk_workspace_bytes(int64_t n_docs, int32_t nq, int32_t k);
+/* The k best accessible documents of each of nq queries.
+ *   d_tokens       concatenated term ids of all queries (device)
+ *   h_offsets      nq + 1 non-decreasing offsets into d_tokens (HOST)
+ *   d_access_mask  optional [n_mask_rows][mask_stride_words] uint32 bitmask in rpx_index_topk's layout; query q uses
+ *                  row h_mask_rows[q] (HOST), so the queries of one theorem can share a row.  NULL: every document.
+ *   d_out_scores64, d_out_idx  [nq, k]; d_out_count optional [nq] = min(k, accessible documents).  Slots past the
+ *                  count hold score -inf, index -1.
+ * The host arrays are copied before the call returns.  One query's result does not depend on the others in the call. */
+int rpx_bm25_topk(const rpx_bm25* ix, const int32_t* d_tokens, const int64_t* h_offsets, int32_t nq,
+                  const uint32_t* d_access_mask, int64_t mask_stride_words, const int32_t* h_mask_rows,
+                  int32_t n_mask_rows, int32_t k, double* d_out_scores64, int64_t* d_out_idx, int32_t* d_out_count,
+                  void* d_workspace, size_t workspace_bytes, void* stream);
+/* get_batch_scores over every document: d_out [n_docs] fp64 scores of the one query d_tokens[0, n_tokens). */
+int rpx_bm25_scores(const rpx_bm25* ix, const int32_t* d_tokens, int64_t n_tokens, double* d_out, void* stream);
+
 /* ------------------------------------------------------------------- test utilities
  * Debug timeline: while `d_stamps` (device, n_slots x 8 uint64) is set, every launch of the 1-CTA GEMM
  * kernel takes the next slot and its CTA 0 records %globaltimer at: kernel entry, prologue done,

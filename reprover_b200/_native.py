@@ -110,6 +110,14 @@ _SIGNATURES = {
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rpx_topk_merge_packed": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p]),
+    "rpx_bm25_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int64,
+                                  C.POINTER(C.c_void_p)]),
+    "rpx_bm25_destroy": (C.c_int, [C.c_void_p]),
+    "rpx_bm25_topk_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32]),
+    "rpx_bm25_topk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                C.c_void_p]),
+    "rpx_bm25_scores": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "rpx_debug_set_timeline": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_gemm_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p]),

@@ -156,21 +156,24 @@ def _stand_in(module: str, name: str) -> type:
     return cls
 
 
+_COMMON_CLASSES = ("IndexedCorpus", "Corpus", "File", "Premise", "Context")
+
+
 @contextlib.contextmanager
 def _reference_classes():
-    """Yield {"IndexedCorpus", "Corpus", "File", "Premise", "Pos"} -> classes that pickle under the
+    """Yield {"IndexedCorpus", "Corpus", "File", "Premise", "Context", "Pos"} -> classes that pickle under the
     reference's names."""
     common = sys.modules.get("common")
     lean_dojo = sys.modules.get("lean_dojo")
     if (common is not None and lean_dojo is not None and hasattr(lean_dojo, "Pos")
-            and all(hasattr(common, n) for n in ("IndexedCorpus", "Corpus", "File", "Premise"))):
-        yield {n: getattr(common, n) for n in ("IndexedCorpus", "Corpus", "File", "Premise")} | {"Pos": lean_dojo.Pos}
+            and all(hasattr(common, n) for n in _COMMON_CLASSES)):
+        yield {n: getattr(common, n) for n in _COMMON_CLASSES} | {"Pos": lean_dojo.Pos}
         return
     added = []
     try:
-        classes = {n: _stand_in("common", n) for n in ("IndexedCorpus", "Corpus", "File", "Premise")}
+        classes = {n: _stand_in("common", n) for n in _COMMON_CLASSES}
         classes["Pos"] = _stand_in("lean_dojo", "Pos")
-        for mod_name, names in (("common", ("IndexedCorpus", "Corpus", "File", "Premise")), ("lean_dojo", ("Pos",))):
+        for mod_name, names in (("common", _COMMON_CLASSES), ("lean_dojo", ("Pos",))):
             if mod_name in sys.modules:
                 raise RuntimeError(f"a module named {mod_name!r} that is not the reference's is loaded; cannot write "
                                    f"the reference index layout from this process")
@@ -192,6 +195,15 @@ def _raw(cls: type, **attrs) -> Any:
     return obj
 
 
+def _ref_pos(ref: Dict[str, type], p: Pos) -> Any:
+    return _raw(ref["Pos"], line_nb=int(p.line_nb), column_nb=int(p.column_nb))
+
+
+def _ref_premise(ref: Dict[str, type], p: Premise) -> Any:
+    return _raw(ref["Premise"], path=p.path, full_name=p.full_name, start=_ref_pos(ref, p.start),
+                end=_ref_pos(ref, p.end), code=p.code)
+
+
 def dump_reference_index(corpus: Corpus, embeddings, fh) -> None:
     """Write `IndexedCorpus(corpus, embeddings)` to the binary file `fh` in the reference's layout."""
     import networkx as nx
@@ -205,9 +217,7 @@ def dump_reference_index(corpus: Corpus, embeddings, fh) -> None:
         def premise(p: Premise):
             q = conv.get(id(p))
             if q is None:
-                q = _raw(ref["Premise"], path=p.path, full_name=p.full_name,
-                         start=_raw(ref["Pos"], line_nb=int(p.start.line_nb), column_nb=int(p.start.column_nb)),
-                         end=_raw(ref["Pos"], line_nb=int(p.end.line_nb), column_nb=int(p.end.column_nb)), code=p.code)
+                q = _ref_premise(ref, p)
                 conv[id(p)] = q
             return q
 
@@ -222,3 +232,27 @@ def dump_reference_index(corpus: Corpus, embeddings, fh) -> None:
         ref_corpus = _raw(ref["Corpus"], transitive_dep_graph=g, all_premises=[premise(p) for p in corpus.all_premises],
                           imported_premises_cache={})
         pickle.dump(_raw(ref["IndexedCorpus"], corpus=ref_corpus, embeddings=emb), fh, protocol=4)
+
+
+def dump_reference_predictions(preds: List[Dict[str, Any]], fh) -> None:
+    """Write retrieval predictions (the records of the reference's BM25 script, retrieval/bm25/main.py:55-67) to the
+    binary file `fh` with `context` as `common.Context`, premises as `common.Premise` and positions as `lean_dojo.Pos`,
+    so that the reference's `retrieval/evaluate.py` and `generation/datamodule.py` load them."""
+    with _reference_classes() as ref:
+        conv: Dict[int, Any] = {}
+
+        def premise(p: Premise):
+            q = conv.get(id(p))
+            if q is None:
+                q = conv[id(p)] = _ref_premise(ref, p)
+            return q
+
+        out = []
+        for rec in preds:
+            ctx = rec["context"]
+            out.append({**rec,
+                        "context": _raw(ref["Context"], path=ctx.path, theorem_full_name=ctx.theorem_full_name,
+                                        theorem_pos=_ref_pos(ref, ctx.theorem_pos), state=ctx.state),
+                        "all_pos_premises": [premise(p) for p in rec["all_pos_premises"]],
+                        "retrieved_premises": [premise(p) for p in rec["retrieved_premises"]]})
+        pickle.dump(out, fh)

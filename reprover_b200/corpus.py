@@ -446,6 +446,19 @@ class Corpus:
         recent[key] = words
         return words
 
+    def accessible_index_mask_words(self, path: str, pos: Any) -> np.ndarray:
+        """The bits of `get_accessible_premise_indexes(path, pos)` in `accessible_mask_words`' layout: premises of the
+        (transitively) imported files and premises of `path` that end at or before `pos`, chosen by index.  Unlike
+        `accessible_mask_words` it does not add same-named duplicates of visible premises; this is the set the
+        reference's BM25 script ranks (retrieval/bm25/main.py:38-40)."""
+        pos = Pos.from_any(pos)
+        words = self._import_mask_words(path).copy()
+        lo, hi = self._range[path]
+        for i in range(lo, hi):
+            if self.all_premises[i].end <= pos:
+                words[i >> 5] |= np.uint32(1 << (i & 31))
+        return words
+
     def accessible_mask_words_range(self, path: str, pos: Any, lo: int, hi: int) -> np.ndarray:
         """The bits [lo, hi) of `accessible_mask_words`, re-packed from bit 0: the bitmask a rank that owns
         rows [lo, hi) of a row-sharded index hands to `rpx_sim_topk` (bit i <=> global row lo + i)."""
