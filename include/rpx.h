@@ -301,13 +301,9 @@ int rpx_debug_set_timeline(unsigned long long* d_stamps, int32_t n_slots);
  * C[M, N] (fp32, ldc = N) = A[M, K] * B[N, K]^T, bf16 inputs; K % 64 == 0, N % 32 == 0. */
 int rpx_gemm_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                       int32_t K, void* stream);
-/* Same contract through the single-CTA 128 x 128 core that runs QKV, O-proj and FFN-down on the
- * throughput path and every GEMM of the latency path. */
+/* Same contract through the 128 x 128 tiles of the core that runs QKV on the throughput path, every GEMM
+ * of the latency path and the similarity stages of the top-k. */
 int rpx_gemm1_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
-                       int32_t K, void* stream);
-/* Same contract through the paired form of the core: clusters of two CTAs on vertically adjacent
- * 128 x 128 tiles that share each B tile through TMA multicast. */
-int rpx_gemm2_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                        int32_t K, void* stream);
 
 enum { RPX_EGEMM_QKV = 0, RPX_EGEMM_OPROJ = 1, RPX_EGEMM_FFN_UP = 2, RPX_EGEMM_FFN_DOWN = 3 };

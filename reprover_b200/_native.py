@@ -123,8 +123,6 @@ _SIGNATURES = {
                                     C.c_void_p]),
     "rpx_gemm1_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                      C.c_void_p]),
-    "rpx_gemm2_bf16_f32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                     C.c_void_p]),
     "rpx_debug_encoder_gemm": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                          C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -270,7 +270,7 @@ struct PdlScope {
 int ss_parts(int d_model, bool latency) { return ceil_div(d_model, latency ? 32 : 128); }
 
 // The encoder's four GEMMs, each on the tiles the forward pass uses for T tokens on the throughput or the
-// latency path.  forward(), forward_latency_layer() and rpx_debug_encoder_gemm all launch through these, so the
+// latency path.  forward_layer() and rpx_debug_encoder_gemm both launch through these, so the
 // epilogue tests run exactly the launches an encode call runs.  A is [T, K], B is [N, K] (packed weights).
 
 // out [T, N] = bf16(A B^T * rs[m]).  On the latency path the CTAs the GEMM leaves idle fetch `prefetch` into L2.
@@ -279,9 +279,9 @@ int qkv_gemm(bool latency, int T, const void* A, const void* B, int N, int K, co
   EpiStoreBF16::Params ep{out, N, rs};
   if (!latency) return launch_gemm<kBlockN, EpiStoreBF16>(A, K, B, K, T, N, K, ep, st);
   if (T <= kLatSmallMMaxTokens)
-    return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st, 0,
+    return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st,
                                                                                              prefetch, prefetch_bytes);
-  return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatStages>(A, K, B, K, T, N, K, ep, st, 0, prefetch, prefetch_bytes);
+  return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatStages>(A, K, B, K, T, N, K, ep, st, prefetch, prefetch_bytes);
 }
 
 // h32 [T, N] += A B^T, h16 = bf16(h32), ss_out = partial sums of h32^2 ([ss_parts(N)][T]).
@@ -339,17 +339,18 @@ int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K,
   return launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(A, K, B, K, T, N, K, ep, st);
 }
 
-int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, const void* next_weights,
-                          size_t next_bytes, int T, int S, int max_len, cudaStream_t st) {
+// One encoder block on the throughput or the latency path, each kernel under its profiling class.
+// `next_weights` (latency path, not the last layer; else null): the QKV projection occupies 18 x ceil(T/64) (or
+// 18 x ceil(T/128)) SMs for 6 heads, and the rest of the GPU fetches these `next_bytes` into L2.
+int forward_layer(rpx_encoder* e, bool latency, const Workspace& ws, const LayerW& w, const void* next_weights,
+                  size_t next_bytes, int T, int S, int max_len, cudaStream_t st) {
   const rpx_t5_config& c = e->cfg;
-  const int D = c.d_model, inner = e->inner, F = c.d_ff, P = e->n_parts_lat;
+  const int D = c.d_model, inner = e->inner, F = c.d_ff, P = latency ? e->n_parts_lat : e->n_parts;
   const float inv_d = 1.0f / (float)D;
   {
     Prof p(e, st, 1);
-    // the QKV projection occupies 18 x ceil(T/64) (or 18 x ceil(T/128)) SMs for 6 heads: the rest of the GPU
-    // fetches the next layer's weights into L2
-    RPX_TRY(qkv_gemm(true, T, ws.h16, w.qkv, 3 * inner, D, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}, ws.qkv, next_weights,
-                     next_bytes, st));
+    RPX_TRY(qkv_gemm(latency, T, ws.h16, w.qkv, 3 * inner, D, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}, ws.qkv,
+                     next_weights, next_bytes, st));
   }
   {
     Prof p(e, st, 2);
@@ -358,15 +359,15 @@ int forward_latency_layer(rpx_encoder* e, const Workspace& ws, const LayerW& w, 
   }
   {
     Prof p(e, st, 3);
-    RPX_TRY(oproj_gemm(true, T, ws.attn, w.o, D, inner, ws.h32, ws.h16, ws.ssB, st));
+    RPX_TRY(oproj_gemm(latency, T, ws.attn, w.o, D, inner, ws.h32, ws.h16, ws.ssB, st));
   }
   {
     Prof p(e, st, 4);
-    RPX_TRY(ffn_up_gemm(true, T, ws.h16, w.wi, 2 * F, D, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}, ws.ffn, st));
+    RPX_TRY(ffn_up_gemm(latency, T, ws.h16, w.wi, 2 * F, D, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}, ws.ffn, st));
   }
   {
     Prof p(e, st, 5);
-    RPX_TRY(ffn_down_gemm(true, T, ws.ffn, w.wo, D, F, ws.h32, ws.h16, ws.ssA, st));
+    RPX_TRY(ffn_down_gemm(latency, T, ws.ffn, w.wo, D, F, ws.h32, ws.h16, ws.ssA, st));
   }
   return RPX_OK;
 }
@@ -385,7 +386,6 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutK
   // the latency path needs d_ff in 128-unit blocks for its split-B tiles (validate_cfg) and narrow-tile n
   const bool latency = T <= e->latency_tokens && D % 32 == 0 && (3 * inner) % 32 == 0;
   const int P = latency ? e->n_parts_lat : e->n_parts;
-  const float inv_d = 1.0f / (float)D;
   PdlScope pdl_scope(latency || T <= kPdlMaxTokens);
   {
     Prof p(e, st, 0);
@@ -399,36 +399,9 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutK
   };
   RPX_TRY(dump(0));
   for (int l = 0; l < c.num_layers; ++l) {
-    const LayerW& w = e->layers[l];
-    if (latency) {
-      const bool has_next = l + 1 < c.num_layers;
-      RPX_TRY(forward_latency_layer(e, ws, w, has_next ? e->layers[l + 1].qkv : nullptr, has_next ? e->layer_bytes : 0, T, S,
-                                    max_len, st));
-      RPX_TRY(dump(l + 1));
-      continue;
-    }
-    {
-      Prof p(e, st, 1);
-      RPX_TRY(qkv_gemm(false, T, ws.h16, w.qkv, 3 * inner, D, RowScale{ws.ssA, P, T, inv_d, c.ln_eps}, ws.qkv, nullptr, 0,
-                       st));
-    }
-    {
-      Prof p(e, st, 2);
-      RPX_TRY(launch_t5_attention(ws.qkv, ws.attn, ws.cu_tokens, e->bias_lut, T, S, max_len, c.num_heads, c.d_kv,
-                                  c.rel_max_distance, st));
-    }
-    {
-      Prof p(e, st, 3);
-      RPX_TRY(oproj_gemm(false, T, ws.attn, w.o, D, inner, ws.h32, ws.h16, ws.ssB, st));
-    }
-    {
-      Prof p(e, st, 4);
-      RPX_TRY(ffn_up_gemm(false, T, ws.h16, w.wi, 2 * F, D, RowScale{ws.ssB, P, T, inv_d, c.ln_eps}, ws.ffn, st));
-    }
-    {
-      Prof p(e, st, 5);
-      RPX_TRY(ffn_down_gemm(false, T, ws.ffn, w.wo, D, F, ws.h32, ws.h16, ws.ssA, st));
-    }
+    const bool prefetch = latency && l + 1 < c.num_layers;
+    RPX_TRY(forward_layer(e, latency, ws, e->layers[l], prefetch ? e->layers[l + 1].qkv : nullptr,
+                          prefetch ? e->layer_bytes : 0, T, S, max_len, st));
     RPX_TRY(dump(l + 1));
   }
   if (kind == OutKind::kHidden) {

@@ -3,7 +3,7 @@
 //
 //   D[M, N] (fp32) = A[M, K] * B[N, K]^T        A, B bf16, K contiguous
 //
-// Structure (one persistent CTA per SM, 160 + 32 * Epi::kWarps threads):
+// Structure (one persistent CTA per SM, 288 threads):
 //   warps 0-3   : MMA warpgroup  — wgmma.mma_async (M = 64 per instruction, one instruction per
 //                 64-row half of the tile, N = BLOCK_N, K = 16) x4 per stage, the fp32 accumulator in
 //                 registers; a stage goes back to the producer (`empty[]`) once the wgmma group that read
@@ -11,7 +11,7 @@
 //                 tile (`acc`, one row of BLOCK_N floats per output row) and published (`tfull`).
 //   warp 4      : TMA producer   — cp.async.bulk.tensor A/B tiles into a STAGES-deep
 //                 128B-swizzled shared-memory ring, completion on `full[]` mbarriers
-//   warps 5..   : epilogue       — read the accumulator tile (one row per thread) and run the fused
+//   warps 5-8   : epilogue       — read the accumulator tile (one row per thread) and run the fused
 //                 epilogue functor; `tempty` hands the tile back.  The MMA warpgroup runs the mainloop of
 //                 tile i+1 while the epilogue works on tile i; it only waits for `tempty` before it writes
 //                 the next accumulator.
@@ -25,6 +25,8 @@
 // query block, B the streamed corpus, and a grid that is a multiple of tiles_m
 // pins every CTA to one query block for its whole life.
 //
+// rpx_gemm_launch.cuh::launch_gemm is the one host launcher of this kernel.
+//
 // The reference has no counterpart: it calls torch `@` / nn.Linear (cuBLAS) —
 // SURVEY.md §2.1 K3/K8/K9/K11.
 #pragma once
@@ -35,15 +37,11 @@ namespace rpx {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle atom row
 constexpr int kMmaK = 16;
-#ifndef RPX_EPI_WARPS
-#define RPX_EPI_WARPS 4
-#endif
 constexpr int kMmaThreads = 128;  // warps 0-3: the MMA warpgroup
 constexpr int kProducerWarp = 4;
 constexpr int kEpiWarp0 = 5;      // first epilogue warp
-// threads of a launch: MMA warpgroup + TMA warp + Epi::kWarps epilogue warps (4 or 8)
-template <class Epi>
-constexpr int gemm_threads() { return kMmaThreads + 32 + 32 * Epi::kWarps; }
+constexpr int kEpiThreads = 128;  // warps 5-8: one warp per 32 (or 16) rows of the tile
+constexpr int kGemmThreads = kMmaThreads + 32 + kEpiThreads;  // 288
 
 template <int BLOCK_N, int STAGES, int BM = kBlockM>
 struct GemmCfg {
@@ -91,9 +89,6 @@ struct TileCtx {
   int row;         // this thread's row inside the tile, 0..127
   int m_blk, n_blk;
   int M, N;
-  int next_m0, next_n0;  // origin of the next tile this CTA will process (next_m0 < 0: none)
-  int next_cols;         // its width
-  int part, split;       // this warp handles the 32-column chunks with (chunk % split) == part
   int rows_per_warp;     // tile rows held by one lane group: 32 (M = 128 tiles) or 16 (M = 64: lanes 16-31 idle)
 };
 
@@ -112,10 +107,7 @@ RPX_DEVICE void acc_ld32(const float* src, uint32_t (&v)[32]) {
 // Epi must provide:
 //   struct Params;                       (trivially copyable kernel argument)
 //   static constexpr size_t kSmemBytes;  (extra dynamic shared memory, may be 0)
-//   static constexpr int kWarps;         (4 or 8 epilogue warps; with 8, two warps share a lane
-//                                         group and split the tile's 32-column chunks between them)
-//   __device__ Epi(const Params&, uint8_t* smem_extra, int row /*tile row this thread owns, 0..127*/,
-//                  int part /*column share of this warp, 0..kWarps/4-1*/);
+//   __device__ Epi(const Params&, uint8_t* smem_extra, int row /*tile row this thread owns, 0..127*/);
 //   __device__ void before_wait(const TileCtx&);  (work that may run while the MMAs of this tile are
 //                                                  still in flight, e.g. prefetching)
 //   __device__ void tile(const TileCtx&);     (all epilogue threads, warp-converged)
@@ -126,25 +118,17 @@ RPX_DEVICE void acc_ld32(const float* src, uint32_t (&v)[32]) {
 // (units u0 = t * BLOCK_N/2) takes rows 256 (u0/128) + u0 % 128 and the same + 128; tmB must then be encoded
 // with a box of BLOCK_N/2 rows.
 //
-// PAIR: the kernel runs as clusters of two CTAs that work in lockstep on vertically adjacent tiles — the same
-// n-tile, m-tiles 2j and 2j+1 — and share the B tile: each CTA's producer loads one half of it (BLOCK_N/2 rows,
-// tmB encoded with that box) and multicasts it into both CTAs, so every B byte crosses L2 once per pair.  A
-// stage is refilled only after the MMA warpgroups of BOTH CTAs have released it (the empty barriers count the
-// peer's arrivals too), since the refill writes into the peer's shared memory as well.  Grid = 2 x pairs.
-//
 // BM = 64 (latency path): 64-row tiles, one wgmma row block.  An epilogue warp then owns 16 rows (row r of the
 // tile belongs to lane r % 16 of lane group r / 16) and its upper 16 lanes idle.  A CTA takes in half the
 // activation bytes per k-block and the ring holds more stages — what a narrow GEMM's time is made of (see
 // rpx_encoder.cu).
-template <int BLOCK_N, int STAGES, class Epi, bool M_FASTEST = false, bool SPLIT_B = false, int BM = kBlockM,
-          bool PAIR = false>
-__global__ void __launch_bounds__(gemm_threads<Epi>(), 1)
+template <int BLOCK_N, int STAGES, class Epi, bool M_FASTEST = false, bool SPLIT_B = false, int BM = kBlockM>
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                int M, int N, int K, int tiles_m, int tiles_n, int n_blk_stride, typename Epi::Params ep,
                L2Prefetch pf) {
   using Cfg = GemmCfg<BLOCK_N, STAGES, BM>;
   constexpr int kSub = BM / 64;  // 64-row wgmma blocks per tile
-  static_assert(!PAIR || (!M_FASTEST && !SPLIT_B), "paired tiles: plain n-fastest order, one B box per CTA");
   if (threadIdx.x == 0) RPX_STAMP(pf, 0);
   if ((int)blockIdx.x >= pf.work_ctas) {
     // Helper CTA (latency path): the GEMM itself keeps only a fraction of the SMs busy, so the launch is
@@ -175,13 +159,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   const int warp = threadIdx.x >> 5;
   const int num_kb = K / kBlockK;
-  // Work units: tiles, or (PAIR) tile pairs; this CTA takes units unit0, unit0 + unit_step, ...
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int num_units = PAIR ? ((tiles_m + 1) / 2) * tiles_n : tiles_m * tiles_n;
-  const int unit0 = PAIR ? (int)blockIdx.x >> 1 : (int)blockIdx.x;
-  const int unit_step = PAIR ? pf.work_ctas >> 1 : pf.work_ctas;
-  auto unit_m = [&](int u) { return PAIR ? 2 * (u / tiles_n) + (int)rank : (M_FASTEST ? u % tiles_m : u / tiles_n); };
-  auto unit_n = [&](int u) { return PAIR ? u % tiles_n : (M_FASTEST ? u / tiles_m : u % tiles_n); };
+  // This CTA takes tiles tile0, tile0 + tile_step, ... of the n-fastest (M_FASTEST: m-fastest) order.
+  const int num_tiles = tiles_m * tiles_n;
+  const int tile0 = (int)blockIdx.x;
+  const int tile_step = pf.work_ctas;
+  auto tile_m = [&](int u) { return M_FASTEST ? u % tiles_m : u / tiles_n; };
+  auto tile_n = [&](int u) { return M_FASTEST ? u / tiles_m : u % tiles_n; };
 
   if (warp == kProducerWarp) {
     if (elect_one()) {
@@ -189,16 +172,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       tma_prefetch_desc(&tmB);
       for (int s = 0; s < STAGES; ++s) {
         mbar_init(&full[s], 1);
-        mbar_init(&empty[s], PAIR ? 2 * kMmaThreads : kMmaThreads);
+        mbar_init(&empty[s], kMmaThreads);
       }
       mbar_init(tfull, kMmaThreads);
-      mbar_init(tempty, 32 * Epi::kWarps);
+      mbar_init(tempty, kEpiThreads);
       fence_mbar_init();
     }
     __syncwarp();
   }
   __syncthreads();
-  if (PAIR) cluster_sync_all();  // the peer's barriers are initialised before anything multicasts or arrives on them
   // Everything above touched only this CTA's shared memory.  Under programmatic dependent launch
   // (rpx_ptx.cuh) the preceding kernel may still be running: the A operand and whatever the epilogue reads
   // from global memory are its outputs and must wait for it (pdl_wait), but the B operand — the weights —
@@ -216,10 +198,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       auto load_b = [&](int st, int n_blk, int kb) {
         if (M_FASTEST) {
           tma_load_2d_hint(sB + st * Cfg::kBBytes, &tmB, &full[st], kb * kBlockK, n_blk * n_blk_stride * BLOCK_N, kEvictFirst);
-        } else if (PAIR) {
-          constexpr int H = BLOCK_N / 2;
-          tma_load_2d_multicast(sB + st * Cfg::kBBytes + rank * H * kBlockK * 2, &tmB, &full[st], kb * kBlockK,
-                                n_blk * BLOCK_N + (int)rank * H, (uint16_t)0x3);
         } else if (SPLIT_B) {
           constexpr int H = BLOCK_N / 2;
           const int u0 = n_blk * H;
@@ -230,8 +208,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           tma_load_2d(sB + st * Cfg::kBBytes, &tmB, &full[st], kb * kBlockK, n_blk * n_blk_stride * BLOCK_N);
         }
       };
-      if (!M_FASTEST && !PAIR && unit0 < num_units) {
-        const int n_blk0 = unit_n(unit0);
+      if (!M_FASTEST && tile0 < num_tiles) {
+        const int n_blk0 = tile_n(tile0);
         pre = num_kb < STAGES ? num_kb : STAGES;
         for (int kb = 0; kb < pre; ++kb) {  // fresh barriers: every stage is free
           mbar_arrive_expect_tx(&full[kb], Cfg::kStageBytes);
@@ -240,9 +218,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       pdl_wait();
       RPX_STAMP(pf, 2);
-      for (int u = unit0; u < num_units; u += unit_step) {
-        const int n_blk = unit_n(u);
-        const int m_blk = unit_m(u);
+      for (int u = tile0; u < num_tiles; u += tile_step) {
+        const int n_blk = tile_n(u);
+        const int m_blk = tile_m(u);
         for (int kb = 0; kb < num_kb; ++kb) {
           if (pre > 0) {
             --pre;  // armed, B in flight: only the A tile is missing
@@ -272,15 +250,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     int stage = 0;
     uint32_t phase = 0;
     uint32_t tphase = 0;
-    auto release = [&](int st) {
-      mbar_arrive(&empty[st]);
-      if (PAIR) mbar_arrive_cluster(&empty[st], rank ^ 1u);
-    };
-    for (int u = unit0; u < num_units; u += unit_step) {
+    for (int u = tile0; u < num_tiles; u += tile_step) {
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
-        if (kb == 0 && u == unit0 && threadIdx.x == 0) RPX_STAMP(pf, 3);
+        if (kb == 0 && u == tile0 && threadIdx.x == 0) RPX_STAMP(pf, 3);
         const uint64_t a_desc = make_smem_desc_kmajor_sw128(smem_u32(sA + stage * Cfg::kABytes));
         const uint64_t b_desc = make_smem_desc_kmajor_sw128(smem_u32(sB + stage * Cfg::kBBytes));
 #pragma unroll
@@ -301,7 +275,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // the group of the previous k-block has retired once at most this one is in flight: its stage is free
         if (kb > 0) {
           wgmma_wait<1>();
-          release(prev);
+          mbar_arrive(&empty[prev]);
         }
         prev = stage;
         if (++stage == STAGES) {
@@ -312,8 +286,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_wait<0>();
 #pragma unroll
       for (int s = 0; s < kSub; ++s) wgmma_fence_operand(acc[s]);
-      release(prev);
-      if (u == unit0 && threadIdx.x == 0) RPX_STAMP(pf, 4);
+      mbar_arrive(&empty[prev]);
+      if (u == tile0 && threadIdx.x == 0) RPX_STAMP(pf, 4);
       // accumulator -> shared memory, once the epilogue has finished reading the previous tile
       mbar_wait(tempty, tphase ^ 1);
       const int r0 = (warp * 16 + (lane >> 2)) * Cfg::kAccStride + 2 * (lane & 3);
@@ -337,14 +311,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // beyond every matrix, so the functors' `m < M` tests switch them off (they read a duplicate row)
     const int row = BM == kBlockM ? lane_grp * 32 + lane : (lane < 16 ? lane_grp * 16 + lane : (1 << 28));
     const int acc_row = BM == kBlockM ? lane_grp * 32 + lane : lane_grp * 16 + (lane & 15);
-    const int part = (warp - kEpiWarp0) >> 2;                 // which share of the columns (0 when 4 warps)
     pdl_wait();  // the epilogue reads (row scales, residual stream) and overwrites the predecessor's outputs
-    Epi epi(ep, smem_extra, lane_grp * 32 + lane, part);      // (the functor's staging is per lane group)
+    Epi epi(ep, smem_extra, lane_grp * 32 + lane);            // (the functor's staging is per lane group)
     uint32_t tphase = 0;
-    for (int u = unit0; u < num_units; u += unit_step) {
+    for (int u = tile0; u < num_tiles; u += tile_step) {
       TileCtx t;
-      t.n_blk = unit_n(u);
-      t.m_blk = unit_m(u);
+      t.n_blk = tile_n(u);
+      t.m_blk = tile_m(u);
       t.m0 = t.m_blk * BM;
       t.rows_per_warp = BM / 4;
       t.n0 = t.n_blk * n_blk_stride * BLOCK_N;  // (n_blk stays the logical tile index)
@@ -352,28 +325,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (n_this > BLOCK_N) n_this = BLOCK_N;
       t.n_cols = n_this;
       t.row = row;
-      t.part = part;
-      t.split = Epi::kWarps / 4;
       t.M = M;
       t.N = N;
       t.acc = sAcc + acc_row * Cfg::kAccStride;
-      {
-        const int nu = u + unit_step;
-        if (nu < num_units) {
-          t.next_m0 = unit_m(nu) * BM;
-          t.next_n0 = unit_n(nu) * BLOCK_N;
-          t.next_cols = N - t.next_n0 < BLOCK_N ? N - t.next_n0 : BLOCK_N;
-        } else {
-          t.next_m0 = -1;
-          t.next_n0 = 0;
-          t.next_cols = 0;
-        }
-      }
       epi.before_wait(t);
       mbar_wait(tfull, tphase);
-      if (threadIdx.x == 32 * kEpiWarp0 && u == unit0) RPX_STAMP(pf, 5);
+      if (threadIdx.x == 32 * kEpiWarp0 && u == tile0) RPX_STAMP(pf, 5);
       epi.tile(t);
-      if (threadIdx.x == 32 * kEpiWarp0 && u == unit0) RPX_STAMP(pf, 6);
+      if (threadIdx.x == 32 * kEpiWarp0 && u == tile0) RPX_STAMP(pf, 6);
       mbar_arrive(tempty);
       tphase ^= 1;
     }
@@ -381,8 +340,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   __syncthreads();
-  // the peer may still multicast into this CTA's ring or arrive on its barriers until it is done too
-  if (PAIR) cluster_sync_all();
   if (threadIdx.x == 0) RPX_STAMP(pf, 7);
 }
 
@@ -424,14 +381,13 @@ struct EpiStoreF32 {
     int ldc;
   };
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = RPX_EPI_WARPS;
   Params p;
-  __device__ EpiStoreF32(const Params& p_, uint8_t*, int, int) : p(p_) {}
+  __device__ EpiStoreF32(const Params& p_, uint8_t*, int) : p(p_) {}
   __device__ void before_wait(const TileCtx&) {}
   __device__ void tile(const TileCtx& t) {
     const int m = t.m0 + t.row;
     const bool ok = m < t.M;
-    for (int c = 32 * t.part; c < t.n_cols; c += 32 * t.split) {
+    for (int c = 0; c < t.n_cols; c += 32) {
       uint32_t v[32];
       acc_ld32(t.acc + c, v);
       if (ok) {
@@ -454,10 +410,9 @@ struct EpiStoreBF16 {
     RowScale rs;
   };
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = RPX_EPI_WARPS;
   Params p;
   float rs = 0.f;  // this thread's row scale for the tile in flight
-  __device__ EpiStoreBF16(const Params& p_, uint8_t*, int, int) : p(p_) {}
+  __device__ EpiStoreBF16(const Params& p_, uint8_t*, int) : p(p_) {}
   // the row scale does not depend on the accumulator: its partial sums (up to 23 L2 round trips on the latency
   // path) are fetched while the MMAs of the tile are still running
   __device__ void before_wait(const TileCtx& t) {
@@ -467,7 +422,7 @@ struct EpiStoreBF16 {
   __device__ void tile(const TileCtx& t) {
     const int m = t.m0 + t.row;
     const bool ok = m < t.M;
-    for (int c = 32 * t.part; c < t.n_cols; c += 32 * t.split) {
+    for (int c = 0; c < t.n_cols; c += 32) {
       uint32_t v[32];
       acc_ld32(t.acc + c, v);
       if (ok) {
@@ -499,7 +454,6 @@ struct EpiStoreBF16 {
 // therefore transposes its 32x32 fp32 block through a swizzled shared-memory tile and does the
 // read-modify-write with lanes running along the row: one instruction covers 4 rows x 128
 // contiguous bytes (4 L1 wavefronts instead of 32).  Residual loads run one chunk ahead.
-// (RPX_EPI_WARPS=8 — two warps per lane group splitting the chunks — is off by default.)
 struct EpiResidualParams {
   float* h32;
   __nv_bfloat16* h16;
@@ -509,16 +463,15 @@ struct EpiResidualParams {
 };
 struct EpiResidualChunkSS {
   using Params = EpiResidualParams;
-  static constexpr int kWarps = RPX_EPI_WARPS;
-  static constexpr size_t kSmemBytes = kWarps * 32 * 32 * sizeof(float);  // one 32x32 tile per warp
+  static constexpr size_t kSmemBytes = (kEpiThreads / 32) * 32 * 32 * sizeof(float);  // one 32x32 tile per warp
   Params p;
   float4* stg;  // this warp's staging tile: row r = 8 float4, stored at slot (j ^ (r & 7))
   int lane, grp;
   float4 h[8];  // residual values of the chunk in flight (loaded one chunk ahead)
-  __device__ EpiResidualChunkSS(const Params& p_, uint8_t* smem_extra, int row, int part) : p(p_) {
+  __device__ EpiResidualChunkSS(const Params& p_, uint8_t* smem_extra, int row) : p(p_) {
     lane = row & 31;
     grp = row >> 5;
-    stg = reinterpret_cast<float4*>(smem_extra) + (part * 4 + grp) * 32 * 8;
+    stg = reinterpret_cast<float4*>(smem_extra) + grp * 32 * 8;
   }
   __device__ __forceinline__ void load_chunk(const TileCtx& t, int c, int row_base, int sub, int col4,
                                              float4 (&hh)[8]) const {
@@ -533,25 +486,22 @@ struct EpiResidualChunkSS {
   // the first chunk's residual values do not depend on the accumulator: they are fetched while the MMAs of
   // the tile are still running (on the latency path that L2 round trip was a third of the epilogue)
   __device__ void before_wait(const TileCtx& t) {
-    const int c = 32 * t.part;
-    if (c < t.n_cols) load_chunk(t, c, t.m0 + grp * t.rows_per_warp, lane >> 3, (lane & 7) * 4, h);
+    if (t.n_cols > 0) load_chunk(t, 0, t.m0 + grp * t.rows_per_warp, lane >> 3, (lane & 7) * 4, h);
   }
   __device__ void tile(const TileCtx& t) {
     const int sub = lane >> 3;        // row within a group of 4
     const int j4 = lane & 7;          // which float4 of the 32-column chunk
     const int col4 = j4 * 4;
     const int row_base = t.m0 + grp * t.rows_per_warp;
-    const int step = 32 * t.split;
     float ss[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) ss[i] = 0.f;
     float4 hn[8];
-    int c = 32 * t.part;
-    for (; c < t.n_cols; c += step) {
+    for (int c = 0; c < t.n_cols; c += 32) {
       uint32_t v[32];
       acc_ld32(t.acc + c, v);
       // next chunk's residual loads go out before this chunk is consumed
-      if (c + step < t.n_cols) load_chunk(t, c + step, row_base, sub, col4, hn);
+      if (c + 32 < t.n_cols) load_chunk(t, c + 32, row_base, sub, col4, hn);
       const size_t col = (size_t)t.n0 + c + col4;
 #pragma unroll
       for (int j = 0; j < 8; ++j)
@@ -620,10 +570,9 @@ struct EpiGeGLUT {
     RowScale rs;
   };
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = RPX_EPI_WARPS;
   Params p;
   float rs = 0.f;  // (fetched ahead of the accumulator: see EpiStoreBF16)
-  __device__ EpiGeGLUT(const Params& p_, uint8_t*, int, int) : p(p_) {}
+  __device__ EpiGeGLUT(const Params& p_, uint8_t*, int) : p(p_) {}
   __device__ void before_wait(const TileCtx& t) {
     const int m = t.m0 + t.row;
     rs = m < t.M ? p.rs.get(m) : 0.f;
@@ -631,7 +580,7 @@ struct EpiGeGLUT {
   __device__ void tile(const TileCtx& t) {
     const int m = t.m0 + t.row;
     const bool ok = m < t.M;
-    for (int c = 32 * t.part; c < HALF; c += 32 * t.split) {
+    for (int c = 0; c < HALF; c += 32) {
       uint32_t g[32], u[32];
       acc_ld32(t.acc + c, g);
       acc_ld32(t.acc + HALF + c, u);

@@ -1,4 +1,5 @@
-// rpx_gemm_launch.cuh — host-side launchers for gemm_tc_kernel and gemm_ws_kernel.
+// rpx_gemm_launch.cuh — the host-side launchers of the two contraction cores: launch_gemm (gemm_tc_kernel, for the
+// encoder's QKV and latency-path GEMMs and the similarity stages) and launch_gemm_ws (gemm_ws_kernel).
 #pragma once
 #include "rpx_common.cuh"
 #include "rpx_gemm.cuh"
@@ -8,16 +9,26 @@ namespace rpx {
 
 constexpr int kGemmStages = 4;
 
-// A: [M, K] bf16 (row pitch lda), B: [N, K] bf16 (row pitch ldb).  K % 64 == 0, N % 32 == 0.
-// `grid_limit` caps the persistent grid (0 = one CTA per SM).
-// M_FASTEST kernels take the grid size verbatim from `grid_limit` (the caller sizes it as a
-// multiple of tiles_m) and accept any N (the epilogue masks the ragged tail).
+// Grid of the similarity stages (M_FASTEST launches, rpx_simtopk.cu).  The kernel sees M = tiles_m * 128 rows while
+// the A map covers only the M real query rows: TMA zero-fills the rest and the epilogue switches them off.
+struct SimGrid {
+  int tiles_m;   // query blocks
+  int tiles_n;   // corpus tiles visited: tiles 0, stride, 2 * stride, ... (the sampling pass) or every tile
+  int stride;
+  int max_ctas;  // persistent grid, a multiple of tiles_m (so every CTA keeps one query block); capped at the tiles
+};
+
+// The one launcher of gemm_tc_kernel.  A: [M, K] bf16 (row pitch lda), B: [N, K] bf16 (row pitch ldb).  K % 64 == 0.
+// Encoder GEMMs (n-fastest): N % 32 == 0, a persistent grid of at most one CTA per SM, launched under PDL when the
+// forward pass enables it, and one slot of the debug timeline each.  `prefetch_ptr`: the SMs the GEMM leaves idle
+// fetch `prefetch_bytes` there into L2.
+// Similarity stages (M_FASTEST): the grid comes from `sim`, any N (the epilogue masks the ragged tail), plain launch.
 template <int BLOCK_N, class Epi, bool M_FASTEST = false, int STAGES = kGemmStages, bool SPLIT_B = false, int BM = kBlockM>
 int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
-                const typename Epi::Params& ep, cudaStream_t stream, int grid_limit = 0, const void* prefetch_ptr = nullptr,
-                size_t prefetch_bytes = 0) {
+                const typename Epi::Params& ep, cudaStream_t stream, const void* prefetch_ptr = nullptr,
+                size_t prefetch_bytes = 0, const SimGrid& sim = SimGrid{}) {
   using Cfg = GemmCfg<BLOCK_N, STAGES, BM>;
-  static_assert(BM == kBlockM || (!M_FASTEST && Epi::kWarps == 4), "64-row tiles: encoder epilogues with one warp per lane group");
+  static_assert(BM == kBlockM || !M_FASTEST, "64-row tiles: encoder GEMMs only");
   RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
   RPX_REQUIRE(K % kBlockK == 0, RPX_ERR_UNSUPPORTED, "gemm: K=%d must be a multiple of %d", K, kBlockK);
   RPX_REQUIRE(M_FASTEST || N % 32 == 0, RPX_ERR_UNSUPPORTED, "gemm: N=%d must be a multiple of 32", N);
@@ -27,8 +38,6 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
   RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BM));
   RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, SPLIT_B ? BLOCK_N / 2 : BLOCK_N));
   RPX_REQUIRE(!SPLIT_B || N % BLOCK_N == 0, RPX_ERR_UNSUPPORTED, "gemm: split-B tiles need N %% %d == 0", BLOCK_N);
-  const int tiles_m = ceil_div(M, BM);
-  const int tiles_n = ceil_div(N, BLOCK_N);
   const size_t smem = Cfg::smem_bytes(Epi::kSmemBytes);
   RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu",
               smem, dev.smem_optin);
@@ -38,13 +47,21 @@ int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, i
     RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured_dev = dev.device;
   }
+  if (M_FASTEST) {
+    const int64_t tiles = (int64_t)sim.tiles_m * sim.tiles_n;
+    const int grid = tiles < sim.max_ctas ? (int)tiles : sim.max_ctas;
+    RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), smem, stream, false, tmA, tmB, sim.tiles_m * BM, N, K,
+                           sim.tiles_m, sim.tiles_n, sim.stride, ep, L2Prefetch{nullptr, 0u, grid, nullptr}));
+    return RPX_OK;
+  }
+  const int tiles_m = ceil_div(M, BM);
+  const int tiles_n = ceil_div(N, BLOCK_N);
   int grid = tiles_m * tiles_n;
-  int cap = grid_limit > 0 ? grid_limit : dev.num_sms;
-  if (grid > cap) grid = cap;
+  if (grid > dev.num_sms) grid = dev.num_sms;
   L2Prefetch pf{prefetch_ptr, (uint32_t)prefetch_bytes, grid, next_timeline_slot()};
   if (prefetch_ptr != nullptr && prefetch_bytes > 0 && prefetch_bytes < ((size_t)1 << 32) && grid < dev.num_sms)
     grid = dev.num_sms;  // surplus SMs run prefetch helpers
-  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(gemm_threads<Epi>()), smem, stream, pdl_enabled(), tmA, tmB, M, N, K, tiles_m,
+  RPX_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(kGemmThreads), smem, stream, pdl_enabled(), tmA, tmB, M, N, K, tiles_m,
                          tiles_n, 1, ep, pf));
   return RPX_OK;
 }
@@ -104,51 +121,6 @@ int launch_gemm_ws(const void* A, int64_t lda, const void* B, int64_t ldb, int M
   if (clusters > max_clusters) clusters = max_clusters;
   RPX_CUDA_OK(launch_pdl<CLUSTER>(kern, dim3(CLUSTER * clusters), dim3(kWsThreads), smem, stream, pdl_enabled(), tmA,
                                   tmB, tmR, M, N, K, tiles_m, tiles_n, ep));
-  return RPX_OK;
-}
-
-// Paired form (gemm_tc_kernel<..., PAIR>): clusters of two CTAs on vertically adjacent 128 x 128 tiles that
-// share each B tile through TMA multicast; persistent over num_sms / 2 pairs.
-template <class Epi, int STAGES = kGemmStages>
-int launch_gemm_pair(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
-                     const typename Epi::Params& ep, cudaStream_t stream) {
-  constexpr int BLOCK_N = 128;
-  using Cfg = GemmCfg<BLOCK_N, STAGES, kBlockM>;
-  RPX_REQUIRE(M > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "gemm: empty problem M=%d N=%d K=%d", M, N, K);
-  RPX_REQUIRE(K % kBlockK == 0, RPX_ERR_UNSUPPORTED, "gemm: K=%d must be a multiple of %d", K, kBlockK);
-  RPX_REQUIRE(N % 32 == 0, RPX_ERR_UNSUPPORTED, "gemm: N=%d must be a multiple of 32", N);
-  DeviceInfo dev;
-  RPX_TRY(get_device_info(&dev));
-  CUtensorMap tmA, tmB;
-  RPX_TRY(make_tmap_bf16_2d(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, kBlockM));
-  RPX_TRY(make_tmap_bf16_2d(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, BLOCK_N / 2));
-  const int tiles_m = ceil_div(M, kBlockM);
-  const int tiles_n = ceil_div(N, BLOCK_N);
-  const size_t smem = Cfg::smem_bytes(Epi::kSmemBytes);
-  RPX_REQUIRE(smem <= dev.smem_optin, RPX_ERR_UNSUPPORTED, "gemm: needs %zu B smem, device allows %zu", smem,
-              dev.smem_optin);
-  auto kern = gemm_tc_kernel<BLOCK_N, STAGES, Epi, false, false, kBlockM, true>;
-  static thread_local int configured_dev = -1;
-  if (configured_dev != dev.device) {
-    RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured_dev = dev.device;
-  }
-  int pairs = ceil_div(tiles_m, 2) * tiles_n;
-  if (pairs > dev.num_sms / 2) pairs = dev.num_sms / 2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(gemm_threads<Epi>());
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  RPX_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, tiles_m, tiles_n, 1, ep,
-                                 L2Prefetch{nullptr, 0u, 2 * pairs, next_timeline_slot()}));
   return RPX_OK;
 }
 

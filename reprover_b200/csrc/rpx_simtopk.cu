@@ -3,7 +3,7 @@
 //     similarities = ctx_emb @ premise_emb.T        (:307)
 //     argsort(descending) ... first k accessible    (:308-322)
 //
-// Stage 1  sim_topk (gemm_tc_kernel<..., EpiSimTopk, M_FASTEST>):
+// Stage 1  sim_topk (gemm_tc_kernel<..., EpiSimTopk, M_FASTEST>, launched by launch_gemm):
 //   wgmma of a 128-query block against 128-premise tiles streamed once from HBM
 //   by TMA; the [Q, N] score matrix is never written.  Each epilogue thread owns one
 //   query row of the accumulator tile, compares its 128 scores against that query's running threshold
@@ -66,7 +66,6 @@ struct EpiSimTopk {
   static_assert(KEEP + SLACK + 32 <= CAP, "list too small");
   using Params = SimTopkParams;
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = 4;  // one warp per lane group: a query's list has one writer
 
   Params p;
   float thr;        // pass rule: score > thr
@@ -78,7 +77,7 @@ struct EpiSimTopk {
   bool published = false;  // this list has contributed to gmin
   bool have_gmin = false;  // the all-CTA bound has been adopted
 
-  __device__ EpiSimTopk(const Params& p_, uint8_t*, int row, int) : p(p_) {
+  __device__ EpiSimTopk(const Params& p_, uint8_t*, int row) : p(p_) {
     lane = row & 31;
     const int cta = blockIdx.x;
     q = (cta % p.tiles_m) * kBlockM + row;
@@ -308,9 +307,8 @@ struct EpiSampleScores {
     int n;
   };
   static constexpr size_t kSmemBytes = 0;
-  static constexpr int kWarps = 4;
   Params p;
-  __device__ EpiSampleScores(const Params& p_, uint8_t*, int, int) : p(p_) {}
+  __device__ EpiSampleScores(const Params& p_, uint8_t*, int) : p(p_) {}
   __device__ void before_wait(const TileCtx&) {}
   __device__ void tile(const TileCtx& t) {
     const int q = t.m0 + t.row;
@@ -823,33 +821,16 @@ int plan_sim(int nq, int k, int d, int num_sms, SimPlan* pl) {
   return RPX_OK;
 }
 
-// Launch of stage 1 with the plan's (fixed) tiles_m / grid.  The A tensor map covers the true
-// nq rows, so query rows beyond nq are zero-filled by TMA and flagged inactive in the epilogue.
+// Stages 0 and 1 on the plan's (fixed) tiles_m / grid.  The A tensor map covers the true nq rows, so query rows
+// beyond nq are zero-filled by TMA and flagged inactive in the epilogue.
 // `tiles_n_override` / `stride`: visit only tiles 0, stride, 2*stride, ... (the sampling pass).
 template <class Epi>
 int launch_sim_epi(const __nv_bfloat16* Q, int nq, const __nv_bfloat16* E, int64_t n, int d,
                    const typename Epi::Params& ep, const SimPlan& pl, cudaStream_t st, int tiles_n_override = 0,
                    int stride = 1) {
-  using Cfg = GemmCfg<kSimBlockN, kGemmStages>;
-  DeviceInfo dev;
-  RPX_TRY(get_device_info(&dev));
-  CUtensorMap tmA, tmB;
-  RPX_TRY(make_tmap_bf16_2d(&tmA, Q, (uint64_t)nq, (uint64_t)d, (uint64_t)d, kBlockM));
-  RPX_TRY(make_tmap_bf16_2d(&tmB, E, (uint64_t)n, (uint64_t)d, (uint64_t)d, kSimBlockN));
   const int tiles_n = tiles_n_override > 0 ? tiles_n_override : (int)ceil_div64(n, kSimBlockN);
-  const size_t smem = Cfg::smem_bytes(Epi::kSmemBytes);
-  auto kern = gemm_tc_kernel<kSimBlockN, kGemmStages, Epi, true>;
-  static thread_local int configured_dev = -1;
-  if (configured_dev != dev.device) {
-    RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured_dev = dev.device;
-  }
-  int64_t tiles = (int64_t)pl.tiles_m * tiles_n;
-  const int grid = tiles < pl.grid ? (int)tiles : pl.grid;  // stays a multiple of tiles_m
-  kern<<<grid, gemm_threads<Epi>(), smem, st>>>(tmA, tmB, pl.tiles_m * kBlockM, (int)n, d, pl.tiles_m, tiles_n, stride,
-                                                ep, L2Prefetch{nullptr, 0u, grid, nullptr});
-  RPX_CUDA_OK(cudaGetLastError());
-  return RPX_OK;
+  return launch_gemm<kSimBlockN, Epi, true>(Q, d, E, d, nq, (int)n, d, ep, st, nullptr, 0,
+                                            SimGrid{pl.tiles_m, tiles_n, stride, pl.grid});
 }
 
 }  // namespace

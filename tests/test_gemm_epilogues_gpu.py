@@ -1,5 +1,5 @@
 """Every encoder GEMM epilogue, launched exactly as the forward pass launches it (rpx_debug_encoder_gemm runs
-the same tile-shape dispatch as forward() and forward_latency_layer()), on both paths and every tile shape,
+the same tile-shape dispatch as forward_layer()), on both paths and every tile shape,
 against the float64 reference and rounding-aware checker of tests/gemm_ref.py.
 
 Sites: QKV (RMSNorm row scale, bf16 store), O-proj and FFN-down (fp32 residual update, bf16 copy, partial
@@ -223,7 +223,7 @@ def test_chained_launches_under_pdl(rpx_lib, cuda_device, out_dir, first, second
 
 @pytest.mark.parametrize("T", [17, 385])
 def test_latency_qkv_prefetch_helpers_change_nothing(rpx_lib, cuda_device, out_dir, T):
-    """Latency QKV with the next layer's weights to prefetch, as forward_latency_layer runs it: the surplus CTAs
+    """Latency QKV with the next layer's weights to prefetch, as forward_layer runs it: the surplus CTAs
     only read.  Outputs are bit-identical to a run without prefetch, sentinels and the prefetched buffer intact."""
     case = Case("qkv", "byt5_small", T, True, 31, cuda_device)
     _native.check(case.run(rpx_lib))

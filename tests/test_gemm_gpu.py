@@ -13,10 +13,9 @@ pytestmark = pytest.mark.gpu
 ENTRY = "rpx_gemm_bf16_f32"
 
 
-@pytest.fixture(params=["rpx_gemm_bf16_f32", "rpx_gemm1_bf16_f32", "rpx_gemm2_bf16_f32"], autouse=True)
+@pytest.fixture(params=["rpx_gemm_bf16_f32", "rpx_gemm1_bf16_f32"], autouse=True)
 def _entry(request):
-    """Every test runs through the warp-specialised 128 x 256 throughput core, the single-CTA 128 x 128 core and
-    its paired (2-CTA cluster, multicast B) form."""
+    """Every test runs through the warp-specialised 128 x 256 throughput core and the 128 x 128 core."""
     global ENTRY
     ENTRY = request.param
     yield
