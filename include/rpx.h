@@ -214,7 +214,8 @@ int rpx_index_stats(rpx_index* ix, void* stream, float* h_norm_max, float* h_max
                     int64_t* h_n_exact);
 
 /* Path selection flags of rpx_index_topk (0 = automatic: streaming kernel for nq <= 2, tensor-core
- * kernel otherwise, exact pass for k > 200).  The forcing flags exist for parity tests. */
+ * kernel otherwise, exact pass for k > 200).  The forcing flags exist for parity tests; forced
+ * streaming takes 1-2 queries (RPX_ERR_UNSUPPORTED otherwise). */
 enum { RPX_TOPK_AUTO = 0, RPX_TOPK_FORCE_MMA = 1, RPX_TOPK_FORCE_STREAM = 2, RPX_TOPK_FORCE_EXACT = 4 };
 
 /*   d_Q [nq, d] bf16; 1 <= k <= 1024 (k <= 200 on the fast paths).

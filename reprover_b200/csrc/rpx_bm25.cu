@@ -12,13 +12,12 @@
 //
 //   bm25_tile_kernel  grid (tiles, queries).  Scores one (query, tile); then either writes the tile's scores
 //                     (dense row) or selects the tile's k best accessible documents under (score desc, index asc) —
-//                     MSB-first radix select on the monotone fp64 keys, ties cut by index — and writes them sorted.
+//                     select_keys on the monotone fp64 keys, ties cut by index — and writes them sorted.
 //   merge             the tiles' sorted lists go through the k-way merge of the multi-GPU path
 //                     (launch_topk_merge, rpx_simtopk.cu), in rounds when tiles * k exceeds what one merge CTA holds.
 #include <new>
 
 #include "rpx_common.cuh"
-#include "rpx_kernels.cuh"
 #include "rpx_topk_common.cuh"
 
 struct rpx_bm25 {
@@ -97,8 +96,7 @@ __global__ void __launch_bounds__(kThreads) bm25_tile_kernel(const Bm25Params p)
   __shared__ double s[kTile];
   // scoring: the token ranges of one chunk of the query; selection: the selected keys and tile-local indexes
   __shared__ __align__(16) uint8_t aux[kMaxK * (sizeof(uint64_t) + sizeof(uint32_t))];
-  __shared__ int hist[256];
-  __shared__ uint64_t bcast[2];
+  __shared__ SelectSmem sel;
   __shared__ int n_sel;
 
   const int tid = threadIdx.x;
@@ -150,64 +148,30 @@ __global__ void __launch_bounds__(kThreads) bm25_tile_kernel(const Bm25Params p)
     valid = hi - (lo + base) >= kPerThread ? 0xFFFFu : (1u << (hi - (lo + base))) - 1u;
     if (mrow) valid &= (__ldg(mrow + ((lo + base) >> 5)) >> ((lo + base) & 31)) & 0xFFFFu;  // base % 16 == 0
   }
-  uint64_t key[kPerThread];
+  uint64_t key[kPerThread];  // 0 (below every score's key) for documents that are not valid
 #pragma unroll
-  for (int e = 0; e < kPerThread; ++e) key[e] = dkey(s[base + e]);
-  int* redi = hist;
-  const int n_valid = block_reduce<int>(__popc(valid), redi, [](int a, int b) { return a + b; }, 0);
+  for (int e = 0; e < kPerThread; ++e) key[e] = ((valid >> e) & 1u) ? dkey(s[base + e]) : 0ull;
+  const int n_valid = block_reduce<int>(__popc(valid), sel.hist, [](int a, int b) { return a + b; }, 0);
   const int k = p.k;
   uint32_t take = valid;
   if (n_valid > k) {
-    // k-th largest key T among the valid entries, 8 bits at a time; `need` = how many entries equal to T belong
-    uint64_t prefix = 0ull, pmask = 0ull;
-    int need = k;
-    for (int pass = 0; pass < 8; ++pass) {
-      const int shift = 56 - 8 * pass;
-      hist[tid] = 0;  // kThreads == 256 bins
-      __syncthreads();
+    const auto each_key = [&](auto f) {
 #pragma unroll
-      for (int e = 0; e < kPerThread; ++e)
-        if (((valid >> e) & 1u) && (key[e] & pmask) == prefix) atomicAdd(&hist[(int)((key[e] >> shift) & 255ull)], 1);
-      __syncthreads();
-      if (tid < 32) {
-        // lane l holds bins 255 - 8 l ... 248 - 8 l (descending); find the bin where the running count reaches `need`
-        int c[8], sum = 0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          c[i] = hist[255 - 8 * tid - i];
-          sum += c[i];
-        }
-        int incl = sum;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-          const int y = __shfl_up_sync(kFullMask, incl, off);
-          if (tid >= off) incl += y;
-        }
-        int run = incl - sum;
-        if (run < need && incl >= need) {
-          int i = 0;
-          while (run + c[i] < need) run += c[i++];
-          bcast[0] = (uint64_t)(255 - 8 * tid - i);
-          bcast[1] = (uint64_t)run;
-        }
-      }
-      __syncthreads();
-      prefix |= bcast[0] << shift;
-      pmask |= 255ull << shift;
-      need -= (int)bcast[1];
-      __syncthreads();
-    }
-    // take every key above T and the first `need` keys equal to T in index order
+      for (int e = 0; e < kPerThread; ++e) f(key[e]);
+    };
+    const KeyCut cut = select_keys<kThreads>(each_key, 1ull, ~0ull, k, 0, sel);
+    // take every key above lo and of the keys equal to lo the first k - n_above in index order (all of them
+    // when n_above < 0)
+    int need = cut.n_above < 0 ? kTile : k - cut.n_above;
     uint32_t eq = 0;
     take = 0;
 #pragma unroll
     for (int e = 0; e < kPerThread; ++e) {
-      if (!((valid >> e) & 1u)) continue;
-      if (key[e] > prefix) take |= 1u << e;
-      else if (key[e] == prefix) eq |= 1u << e;
+      if (key[e] > cut.lo) take |= 1u << e;
+      else if (key[e] == cut.lo) eq |= 1u << e;
     }
     int n_eq_total;
-    int before = block_exclusive_scan(__popc(eq), hist, &n_eq_total);
+    int before = block_exclusive_scan(__popc(eq), sel.hist, &n_eq_total);
 #pragma unroll
     for (int e = 0; e < kPerThread; ++e)
       if (((eq >> e) & 1u) && before < need) {
@@ -218,7 +182,7 @@ __global__ void __launch_bounds__(kThreads) bm25_tile_kernel(const Bm25Params p)
   uint64_t* sel_key = reinterpret_cast<uint64_t*>(aux);
   uint32_t* sel_idx = reinterpret_cast<uint32_t*>(sel_key + kMaxK);
   int n_taken;
-  int pos = block_exclusive_scan(__popc(take), hist, &n_taken);  // also orders the ranges' last use before reuse
+  int pos = block_exclusive_scan(__popc(take), sel.hist, &n_taken);  // also orders the ranges' last use before reuse
 #pragma unroll
   for (int e = 0; e < kPerThread; ++e)
     if ((take >> e) & 1u) {
@@ -228,24 +192,12 @@ __global__ void __launch_bounds__(kThreads) bm25_tile_kernel(const Bm25Params p)
     }
   if (tid == 0) n_sel = n_taken;
   __syncthreads();
-  // selected entries arrive in index order, so the rank of an entry is the number of larger keys plus the number of
-  // equal keys before it
+  // the list of (tile, query); tile-local indexes, ties broken by index
   const int ns = n_sel;
   const size_t row = ((size_t)blockIdx.x * p.nq + q) * k;
-  for (int c = tid; c < ns; c += kThreads) {
-    const uint64_t kc = sel_key[c];
-    int rank = 0;
-    for (int j = 0; j < ns; ++j) {
-      const uint64_t kj = sel_key[j];
-      rank += (kj > kc || (kj == kc && j < c)) ? 1 : 0;
-    }
-    p.part_s[row + rank] = undkey(kc);
-    p.part_i[row + rank] = lo + sel_idx[c];
-  }
-  for (int r = ns + tid; r < k; r += kThreads) {
-    p.part_s[row + r] = -INFINITY;
-    p.part_i[row + r] = -1;
-  }
+  const TopkOut out{nullptr, p.part_s + row, p.part_i + row, nullptr, nullptr, lo};
+  for (int c = tid; c < ns; c += kThreads) out.put(0, k, rank_desc(sel_key, sel_idx, ns, c), undkey(sel_key[c]), sel_idx[c]);
+  out.pad(0, k, ns, tid, kThreads);
 }
 
 struct Bm25Ws {

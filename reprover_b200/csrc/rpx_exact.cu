@@ -5,7 +5,7 @@
 //     similarities = ctx_emb @ premise_emb.t();  idxs = similarities.argsort(descending=True)
 // (common.py:307-308) with the contract's arithmetic itself: every admissible row is scored with the
 // canonical fp64 dot product and the k best under (score desc, index asc) are selected exactly
-// (radix select on the monotone 64-bit score keys, ties cut by index).
+// (select_keys on the monotone 64-bit score keys, then on the indices of the entries tied at the k-th key).
 //
 //   exact_topk_kernel   cooperative launch, one CTA per SM.  Per query: phase A — all warps stream the
 //                       index (one row per warp trip, 16-byte coalesced loads, fp64 accumulation) and
@@ -14,10 +14,7 @@
 //                       at once (~3 us), which is all the fast paths ever pay for it on ordinary data.
 //   row_norm_max_kernel HBM-bound pass over the index: max_i sum_j E[i,j]^2 -> IndexState::norm2_max
 //                       (the ||e|| factor of the guard's epsilon); runs once per rpx_index_create.
-#include <stdlib.h>
-
 #include "rpx_common.cuh"
-#include "rpx_kernels.cuh"
 #include "rpx_topk_common.cuh"
 
 namespace rpx {
@@ -26,11 +23,6 @@ namespace {
 
 constexpr int kExactThreads = 512;
 constexpr int kExactMaxK = 1024;
-
-struct ExactCand {
-  uint64_t key;  // dkey(fp64 score)
-  uint64_t idx;  // local row
-};
 
 // Sense-reversing grid barrier (all CTAs co-resident: cooperative launch).  `count` returns to zero
 // after every barrier, `gen` only ever increments, so nothing has to be reset between launches.
@@ -60,123 +52,32 @@ struct ExactParams {
   int d, k, nq;
   const uint32_t* mask;
   int64_t mask_stride;
-  float* out_scores;
-  double* out_scores64;
-  int64_t* out_idx;
-  int32_t* out_count;
-  int64_t* out_packed;
-  int64_t idx_offset;
-  IndexState* state;
-  const uint32_t* flagged;
-  const ExactBound* bounds;
-  ExactCand* cand;   // [n]
+  TopkOut out;
+  GuardOut guard;
+  TopkCand* cand;    // [n]
   int all_queries;   // 1: every query 0..nq-1 goes through this path (no guard ran)
 };
-
-__device__ __forceinline__ void write_result(const ExactParams& p, int q, int rank, double score, int64_t idx) {
-  const size_t o = (size_t)q * p.k + rank;
-  p.out_scores[o] = (float)score;
-  if (p.out_scores64) p.out_scores64[o] = score;
-  p.out_idx[o] = idx;
-  if (p.out_packed) {
-    p.out_packed[2 * o] = __double_as_longlong(score);
-    p.out_packed[2 * o + 1] = idx;
-  }
-}
-
-// k-th largest of the C 64-bit keys in cand[] (C > k >= 1), MSB-first 8-bit radix select.
-// Returns the key value T and, in *need_eq, how many entries equal to T belong to the top-k.
-__device__ uint64_t radix_select_desc(const ExactCand* cand, int C, int k, int* hist, uint64_t* bcast, int* need_eq) {
-  uint64_t prefix = 0ull, pmask = 0ull;
-  int need = k;
-  const int tid = threadIdx.x;
-  for (int pass = 0; pass < 8; ++pass) {
-    const int shift = 56 - 8 * pass;
-    for (int b = tid; b < 256; b += kExactThreads) hist[b] = 0;
-    __syncthreads();
-    for (int i = tid; i < C; i += kExactThreads) {
-      const uint64_t key = __ldcg(&cand[i].key);
-      if ((key & pmask) == prefix) atomicAdd(&hist[(int)((key >> shift) & 255ull)], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int cum = 0, dgt = 0;
-      for (int b = 255; b >= 0; --b) {
-        if (cum + hist[b] >= need) {
-          dgt = b;
-          break;
-        }
-        cum += hist[b];
-      }
-      bcast[0] = (uint64_t)dgt;
-      bcast[1] = (uint64_t)cum;
-    }
-    __syncthreads();
-    prefix |= bcast[0] << shift;
-    pmask |= 255ull << shift;
-    need -= (int)bcast[1];
-    __syncthreads();
-  }
-  *need_eq = need;
-  return prefix;
-}
-
-// The `need`-th smallest row index among the entries whose key equals T (there are more than `need`).
-__device__ uint64_t radix_select_idx_asc(const ExactCand* cand, int C, uint64_t T, int need, int* hist, uint64_t* bcast) {
-  uint64_t prefix = 0ull, pmask = 0ull;
-  const int tid = threadIdx.x;
-  for (int pass = 0; pass < 4; ++pass) {
-    const int shift = 24 - 8 * pass;
-    for (int b = tid; b < 256; b += kExactThreads) hist[b] = 0;
-    __syncthreads();
-    for (int i = tid; i < C; i += kExactThreads) {
-      if (__ldcg(&cand[i].key) != T) continue;
-      const uint64_t ix = __ldcg(&cand[i].idx);
-      if ((ix & pmask) == prefix) atomicAdd(&hist[(int)((ix >> shift) & 255ull)], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int cum = 0, dgt = 255;
-      for (int b = 0; b < 256; ++b) {
-        if (cum + hist[b] >= need) {
-          dgt = b;
-          break;
-        }
-        cum += hist[b];
-      }
-      bcast[0] = (uint64_t)dgt;
-      bcast[1] = (uint64_t)cum;
-    }
-    __syncthreads();
-    prefix |= bcast[0] << shift;
-    pmask |= 255ull << shift;
-    need -= (int)bcast[1];
-    __syncthreads();
-  }
-  return prefix;
-}
 
 __global__ void __launch_bounds__(kExactThreads, 1) exact_topk_kernel(ExactParams p) {
   extern __shared__ __align__(16) uint8_t sm_raw[];
   __nv_bfloat16* sq = reinterpret_cast<__nv_bfloat16*>(sm_raw);                                   // [d]
   uint64_t* sel_key = reinterpret_cast<uint64_t*>(sm_raw + (((size_t)p.d * 2 + 15) & ~(size_t)15));  // [kExactMaxK]
   uint32_t* sel_idx = reinterpret_cast<uint32_t*>(sel_key + kExactMaxK);                            // [kExactMaxK]
-  __shared__ int hist[256];
-  __shared__ uint64_t bcast[2];
+  __shared__ SelectSmem sel;
   __shared__ int n_sel;
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int n_f = p.all_queries ? p.nq : (int)*reinterpret_cast<volatile uint32_t*>(&p.state->n_flagged);
+  const int n_f = p.all_queries ? p.nq : (int)*reinterpret_cast<volatile uint32_t*>(&p.guard.state->n_flagged);
   if (n_f == 0) return;
   const int64_t gwarp = (int64_t)blockIdx.x * (kExactThreads / 32) + (tid >> 5);
   const int64_t n_warps = (int64_t)gridDim.x * (kExactThreads / 32);
 
   for (int f = 0; f < n_f; ++f) {
-    const int q = p.all_queries ? f : (int)p.flagged[f];
+    const int q = p.all_queries ? f : (int)p.guard.flagged[f];
     ExactBound bound;
     bound.score = -INFINITY;
     bound.idx = 0x7FFFFFFF;
-    if (!p.all_queries) bound = p.bounds[q];
+    if (!p.all_queries) bound = p.guard.bounds[q];
     const bool unbounded = bound.score == -INFINITY;
     for (int i = tid; i < p.d / 8; i += kExactThreads)
       reinterpret_cast<uint4*>(sq)[i] = reinterpret_cast<const uint4*>(p.Q + (size_t)q * p.d)[i];
@@ -188,71 +89,63 @@ __global__ void __launch_bounds__(kExactThreads, 1) exact_topk_kernel(ExactParam
       const double s = dot64_canonical(sq, p.E + (size_t)row * p.d, p.d, lane);
       const bool keep = unbounded || s > bound.score || (s == bound.score && row <= bound.idx);
       if (lane == 0 && keep) {
-        const uint32_t pos = atomicAdd(&p.state->fb_count, 1u);
-        ExactCand c;
+        const uint32_t pos = atomicAdd(&p.guard.state->fb_count, 1u);
+        TopkCand c;
         c.key = dkey(s);
         c.idx = (uint64_t)row;
         p.cand[pos] = c;
       }
     }
-    grid_barrier(p.state);
+    grid_barrier(p.guard.state);
     // ---- phase B: exact selection + ranking by CTA 0
     if (blockIdx.x == 0) {
-      const int C = (int)*reinterpret_cast<volatile uint32_t*>(&p.state->fb_count);
+      const int C = (int)*reinterpret_cast<volatile uint32_t*>(&p.guard.state->fb_count);
       const int k = p.k;
       if (tid == 0) n_sel = 0;
-      __syncthreads();
-      if (C <= k) {
-        for (int i = tid; i < C; i += kExactThreads) {
-          sel_key[i] = __ldcg(&p.cand[i].key);
-          sel_idx[i] = (uint32_t)__ldcg(&p.cand[i].idx);
+      // the k best: every key above T, and of the keys equal to T those with index <= idx_cut
+      uint64_t T = 0ull, idx_cut = ~0ull;
+      if (C > k) {
+        const auto each_key = [&](auto f) {
+          for (int i = tid; i < C; i += kExactThreads) f(__ldcg(&p.cand[i].key));
+        };
+        const KeyCut cut = select_keys<kExactThreads>(each_key, 0ull, ~0ull, k, 0, sel);
+        T = cut.lo;
+        if (cut.n_above >= 0) {
+          // more entries equal T than the top k has room for: the k - n_above smallest indices among them
+          const auto each_tied = [&](auto f) {
+            for (int i = tid; i < C; i += kExactThreads)
+              if (__ldcg(&p.cand[i].key) == T) f(0xFFFFFFFFull - __ldcg(&p.cand[i].idx));
+          };
+          __syncthreads();  // `sel` is rewritten
+          idx_cut = 0xFFFFFFFFull - select_keys<kExactThreads>(each_tied, 0ull, 0xFFFFFFFFull, k - cut.n_above, 0, sel).lo;
         }
-        if (tid == 0) n_sel = C;
-      } else {
-        int need_eq = 0;
-        const uint64_t T = radix_select_desc(p.cand, C, k, hist, bcast, &need_eq);
-        // how many entries carry exactly the k-th key?
-        int eq = 0;
-        for (int i = tid; i < C; i += kExactThreads) eq += __ldcg(&p.cand[i].key) == T ? 1 : 0;
-        __shared__ int redi[32];
-        eq = block_reduce<int>(eq, redi, [](int a, int b) { return a + b; }, 0);
-        uint64_t idx_cut = ~0ull;  // equals with idx <= idx_cut are taken
-        if (eq > need_eq) idx_cut = radix_select_idx_asc(p.cand, C, T, need_eq, hist, bcast);
-        for (int i = tid; i < C; i += kExactThreads) {
-          const uint64_t key = __ldcg(&p.cand[i].key);
-          if (key < T) continue;
-          const uint64_t ix = __ldcg(&p.cand[i].idx);
-          if (key > T || ix <= idx_cut) {
-            const int pos = atomicAdd(&n_sel, 1);
-            if (pos < kExactMaxK) {
-              sel_key[pos] = key;
-              sel_idx[pos] = (uint32_t)ix;
-            }
+      }
+      __syncthreads();  // n_sel
+      for (int i = tid; i < C; i += kExactThreads) {
+        const uint64_t key = __ldcg(&p.cand[i].key);
+        if (key < T) continue;
+        const uint64_t ix = __ldcg(&p.cand[i].idx);
+        if (key > T || ix <= idx_cut) {
+          const int pos = atomicAdd(&n_sel, 1);
+          if (pos < kExactMaxK) {
+            sel_key[pos] = key;
+            sel_idx[pos] = (uint32_t)ix;
           }
         }
       }
       __syncthreads();
       const int ns = n_sel < k ? n_sel : k;  // == k whenever C > k
-      for (int c = tid; c < ns; c += kExactThreads) {
-        const uint64_t kc = sel_key[c];
-        const uint32_t ic = sel_idx[c];
-        int rank = 0;
-        for (int j = 0; j < ns; ++j) {
-          const uint64_t kj = sel_key[j];
-          rank += (kj > kc || (kj == kc && sel_idx[j] < ic)) ? 1 : 0;
-        }
-        write_result(p, q, rank, undkey(kc), (int64_t)ic + p.idx_offset);
-      }
-      for (int r = ns + tid; r < k; r += kExactThreads) write_result(p, q, r, -INFINITY, -1);
-      if (p.out_count && tid == 0) p.out_count[q] = ns;
+      for (int c = tid; c < ns; c += kExactThreads)
+        p.out.put(q, k, rank_desc(sel_key, sel_idx, ns, c), undkey(sel_key[c]), sel_idx[c]);
+      p.out.pad(q, k, ns, tid, kExactThreads);
       __syncthreads();
-      if (tid == 0) p.state->fb_count = 0u;
+      if (tid == 0) p.guard.state->fb_count = 0u;
     }
-    grid_barrier(p.state);
+    grid_barrier(p.guard.state);
   }
   if (blockIdx.x == 0 && tid == 0) {
-    if (!p.all_queries) p.state->n_flagged = 0u;
-    atomicAdd(&p.state->n_exact_total, (uint32_t)n_f);
+    if (!p.all_queries) p.guard.state->n_flagged = 0u;
+    atomicAdd(&p.guard.state->n_exact_total, (uint32_t)n_f);
   }
 }
 
@@ -293,7 +186,7 @@ __global__ void __launch_bounds__(256) row_norm_max_kernel(const __nv_bfloat16* 
 
 }  // namespace
 
-size_t exact_cand_bytes(int64_t n) { return align_up((size_t)(n > 0 ? n : 1) * sizeof(ExactCand), 256); }
+size_t exact_cand_bytes(int64_t n) { return align_up((size_t)(n > 0 ? n : 1) * sizeof(TopkCand), 256); }
 
 int launch_row_norm_max(const __nv_bfloat16* E, int64_t n, int d, IndexState* state, cudaStream_t st) {
   if (n <= 0) return RPX_OK;
@@ -319,16 +212,9 @@ int launch_exact_topk(const TopkCall& c, void* cand_ws, bool all_queries) {
   p.nq = c.nq;
   p.mask = c.mask;
   p.mask_stride = c.mask_stride;
-  p.out_scores = c.out_scores;
-  p.out_scores64 = c.out_scores64;
-  p.out_idx = c.out_idx;
-  p.out_count = c.out_count;
-  p.out_packed = c.out_packed;
-  p.idx_offset = c.idx_offset;
-  p.state = c.state;
-  p.flagged = c.flagged;
-  p.bounds = c.bounds;
-  p.cand = static_cast<ExactCand*>(cand_ws);
+  p.out = c.out;
+  p.guard = c.guard;
+  p.cand = static_cast<TopkCand*>(cand_ws);
   p.all_queries = all_queries ? 1 : 0;
   const size_t smem = (((size_t)c.d * 2 + 15) & ~(size_t)15) + (size_t)kExactMaxK * (sizeof(uint64_t) + sizeof(uint32_t));
   static thread_local int configured = -1;
@@ -337,19 +223,10 @@ int launch_exact_topk(const TopkCall& c, void* cand_ws, bool all_queries) {
     configured = dev.device;
   }
   RPX_REQUIRE(smem <= 64 * 1024, RPX_ERR_UNSUPPORTED, "exact top-k: d=%d too wide", c.d);
-  static int coop = -1;
-  if (coop < 0) {
-    const char* e = getenv("RPX_EXACT_COOP");  // experiment knob: 0 = plain launch (no co-residency guarantee)
-    coop = (e && e[0] == '0') ? 0 : 1;
-  }
-  if (coop) {
-    void* args[] = {&p};
-    RPX_CUDA_OK(cudaLaunchCooperativeKernel((const void*)exact_topk_kernel, dim3(dev.num_sms), dim3(kExactThreads), args, smem,
-                                            c.st));
-  } else {
-    exact_topk_kernel<<<dev.num_sms, kExactThreads, smem, c.st>>>(p);
-    RPX_CUDA_OK(cudaGetLastError());
-  }
+  // the kernel spins on a grid barrier: its CTAs must be co-resident
+  void* args[] = {&p};
+  RPX_CUDA_OK(cudaLaunchCooperativeKernel((const void*)exact_topk_kernel, dim3(dev.num_sms), dim3(kExactThreads), args, smem,
+                                          c.st));
   return RPX_OK;
 }
 

@@ -8,12 +8,9 @@
 //     nq <= 2            rpx_smallq.cu   one HBM-bound streaming kernel (the reference's real call: nq = 1)
 //     otherwise          rpx_simtopk.cu  wgmma with the top-k fused into the epilogue
 //     k > 200 or flagged rpx_exact.cu    exact fp64 pass (always launched; returns at once if idle)
-#include <stdlib.h>
-
 #include <new>
 
 #include "rpx_common.cuh"
-#include "rpx_kernels.cuh"
 #include "rpx_topk_common.cuh"
 
 struct rpx_index {
@@ -28,20 +25,6 @@ namespace {
 
 constexpr size_t kStateBytes = 256;
 constexpr int kMaxSmsForSizing = 160;  // workspace queries work without a device
-
-int small_q_max() {
-  static int v = -1;
-  if (v < 0) {
-    // Largest nq routed to the streaming kernel (0..4; RPX_SMALLQ_MAX overrides, tools/topk_bench.py times every
-    // path by query count).  One or two queries leave the streaming kernel HBM-bound; from three on it needs a
-    // second pass, and the FMA work of several queries per index byte is what a tensor core is for.
-    const char* e = getenv("RPX_SMALLQ_MAX");
-    v = e ? atoi(e) : 2;
-    if (v < 0) v = 0;
-    if (v > 4) v = 4;
-  }
-  return v;
-}
 
 struct WsLayout {
   size_t flagged, bounds, cand, path, total;
@@ -97,15 +80,8 @@ int topk_dispatch(const rpx_index* ix, const void* d_Q, int32_t nq, int32_t k, c
   c.k = k;
   c.mask = d_access_mask;
   c.mask_stride = mask_stride_words;
-  c.out_scores = d_out_scores;
-  c.out_scores64 = d_out_scores64;
-  c.out_idx = d_out_idx;
-  c.out_count = d_out_count;
-  c.out_packed = d_out_packed;
-  c.idx_offset = idx_offset;
-  c.state = ix->state;
-  c.flagged = reinterpret_cast<uint32_t*>(base + L.flagged);
-  c.bounds = reinterpret_cast<ExactBound*>(base + L.bounds);
+  c.out = TopkOut{d_out_scores, d_out_scores64, d_out_idx, d_out_count, d_out_packed, idx_offset};
+  c.guard = GuardOut{ix->state, reinterpret_cast<uint32_t*>(base + L.flagged), reinterpret_cast<ExactBound*>(base + L.bounds)};
   c.st = static_cast<cudaStream_t>(stream);
   void* cand_ws = base + L.cand;
   void* path_ws = base + L.path;
@@ -115,12 +91,12 @@ int topk_dispatch(const rpx_index* ix, const void* d_Q, int32_t nq, int32_t k, c
   else if (flags & RPX_TOPK_FORCE_STREAM) path = 2;
   else if (flags & RPX_TOPK_FORCE_MMA) path = 1;
   else if (k > kFastPathMaxK) path = 4;
-  else if (ix->n > 0 && nq <= small_q_max() && smallq_supported(nq, k, ix->d)) path = 2;
+  else if (ix->n > 0 && smallq_supported(nq, k, ix->d)) path = 2;
   else path = 1;
   if (path == 2) {
     RPX_REQUIRE(ix->n > 0 && smallq_supported(nq, k, ix->d), RPX_ERR_UNSUPPORTED,
-                "top-k: the streaming path takes 1..4 queries, k <= %d, d <= 2048, n > 0", kFastPathMaxK);
-    RPX_TRY(launch_smallq_topk(c, path_ws, topk_n_res(k)));
+                "top-k: the streaming path takes 1..2 queries, k <= %d, d <= 2048, n > 0", kFastPathMaxK);
+    RPX_TRY(launch_smallq_topk(c, path_ws));
   } else if (path == 1) {
     RPX_REQUIRE(k <= kFastPathMaxK, RPX_ERR_UNSUPPORTED, "top-k: the tensor-core path takes k <= %d", kFastPathMaxK);
     RPX_TRY(run_mma_topk(c, path_ws, workspace_bytes - L.path));

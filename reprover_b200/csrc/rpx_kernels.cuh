@@ -1,5 +1,5 @@
-// rpx_kernels.cuh — launchers of the non-GEMM kernels (defined in rpx_attention.cu,
-// rpx_elementwise.cu, rpx_simtopk.cu).
+// rpx_kernels.cuh — launchers of the encoder's non-GEMM kernels (defined in rpx_attention.cu and
+// rpx_elementwise.cu).  The top-k launchers are declared in rpx_topk_common.cuh.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -45,45 +45,5 @@ int launch_hidden_store(const float* h32, const float* ss, int ss_stride, int n_
 // rows written at dst_row0 + (n / blk) * blk_stride + (n % blk)  (FFN interleave when blk_stride != blk).
 int launch_pack_weight(const float* src, const float* scale, __nv_bfloat16* dst, int n_rows, int n_cols,
                        int dst_row0, int blk, int blk_stride, cudaStream_t stream);
-
-// ---- top-k paths (rpx_simtopk.cu: wgmma, rpx_smallq.cu: HBM streaming, rpx_exact.cu: exact fp64)
-struct IndexState;
-struct ExactBound;
-// One similarity + top-k request (all pointers are device pointers).
-struct TopkCall {
-  const __nv_bfloat16* Q;   // [nq, d]
-  int nq;
-  const __nv_bfloat16* E;   // [n, d]
-  int64_t n;
-  int d, k;
-  const uint32_t* mask;     // optional access bitmask [nq][mask_stride]
-  int64_t mask_stride;
-  float* out_scores;        // [nq, k]
-  double* out_scores64;     // optional [nq, k]
-  int64_t* out_idx;         // [nq, k]
-  int32_t* out_count;       // optional [nq]
-  int64_t* out_packed;      // optional [nq, k, 2]: (fp64 score bits, index) — the all-gather payload
-  int64_t idx_offset;
-  IndexState* state;        // device state of the index handle
-  uint32_t* flagged;        // [nq] guard scratch
-  ExactBound* bounds;       // [nq] guard scratch
-  cudaStream_t st;
-};
-// re-score set size for k results (k + margin; the guard covers what the margin does not)
-inline int topk_n_res(int k) { return k + (k / 8 > 12 ? k / 8 : 12); }
-constexpr int kFastPathMaxK = 200;   // larger k goes through the exact path
-
-int launch_row_norm_max(const __nv_bfloat16* E, int64_t n, int d, IndexState* state, cudaStream_t st);
-size_t exact_cand_bytes(int64_t n);
-int launch_exact_topk(const TopkCall& c, void* cand_ws, bool all_queries);
-bool smallq_supported(int nq, int k, int d);
-size_t smallq_workspace_bytes(int num_sms);
-int launch_smallq_topk(const TopkCall& c, void* ws, int n_res);
-size_t mma_topk_workspace_bytes(int nq, int k, int d, int num_sms);
-int run_mma_topk(const TopkCall& c, void* ws, size_t ws_bytes);
-// k-way merge of per-shard results; `packed`: one [n_parts, nq, k, 2] (score bits, index) buffer.
-int launch_topk_merge(const double* d_scores64, const int64_t* d_idx_or_packed, bool packed, int n_parts, int nq, int k,
-                      float* d_out_scores, double* d_out_scores64, int64_t* d_out_idx, int32_t* d_out_count,
-                      cudaStream_t st);
 
 }  // namespace rpx

@@ -19,7 +19,6 @@
 #include <math.h>
 
 #include "rpx_gemm_launch.cuh"
-#include "rpx_kernels.cuh"
 #include "rpx_topk_common.cuh"
 
 namespace rpx {
@@ -27,14 +26,8 @@ namespace rpx {
 namespace {
 
 constexpr int kSimBlockN = 128;
-#ifndef RPX_SIM_SAMPLE_TILES
-#define RPX_SIM_SAMPLE_TILES 64
-#endif
-#ifndef RPX_SIM_SEL_SLACK
-#define RPX_SIM_SEL_SLACK 16
-#endif
-constexpr int kSampleTiles = RPX_SIM_SAMPLE_TILES;  // 64 x 128 = 8192 sampled premises
-constexpr int kSelSlack = RPX_SIM_SEL_SLACK;        // stage 2 re-scores between n_res and n_res + kSelSlack rows
+constexpr int kSampleTiles = 64;  // 64 x 128 = 8192 sampled premises
+constexpr int kSelSlack = 16;     // stage 2 re-scores between n_res and n_res + kSelSlack rows
 constexpr unsigned kFull = kFullMask;
 
 // EPL = candidate entries per lane: a list holds CAP = 32*EPL entries and is compacted back to
@@ -451,19 +444,14 @@ constexpr int kSelMax = 288;  // >= largest re-score set (k + margin + selection
 __device__ __forceinline__ uint64_t ckey(uint2 e) { return ckey32(e.x, e.y); }
 
 // One CTA per query.  The query's candidate lists (one per stage-1 CTA that served its block,
-// each <= list_max entries) are staged in shared memory as 64-bit composite keys; a bisection
-// picks the `n_res` best (+ <= 16), which are re-scored in fp64 and ranked exactly.  The exactness
+// each <= list_max entries) are staged in shared memory as 64-bit composite keys; select_keys
+// picks the `n_res` best (+ <= kSelSlack), which are re-scored in fp64 and ranked exactly.  The exactness
 // guard (rpx_topk_common.cuh) then compares the k-th re-scored entry with the best fp32 score any
 // row outside the re-scored set can have — the largest final threshold of the query's lists
 // (`thr_out`: everything stage 1 dropped scored at or below it) or the selection threshold — and
 // flags the query for the exact path when the gap is inside the tensor-core error bound.
 struct SelectOut {
-  float* scores;
-  double* scores64;
-  int64_t* idx;
-  int32_t* count;
-  int64_t* packed;
-  int64_t idx_offset;
+  TopkOut out;
   GuardOut guard;
   float guard_coeff;
   int q_base;  // number of query 0 of this launch within the call
@@ -485,8 +473,7 @@ select_rescore_kernel(const uint2* __restrict__ cand, const int32_t* __restrict_
       (reinterpret_cast<uintptr_t>(seg_off + n_seg + 1) + 15) & ~(uintptr_t)15);                   // [n_seg * list_max]
   __shared__ uint64_t red64[32];
   __shared__ float redf[32];
-  __shared__ int hist[256];
-  __shared__ int sel_bin, sel_above;
+  __shared__ SelectSmem sel;
   __shared__ int n_sel;
   __shared__ double kth_score;
   __shared__ uint32_t kth_idx;
@@ -535,58 +522,13 @@ select_rescore_kernel(const uint2* __restrict__ cand, const int32_t* __restrict_
   kmin = block_reduce<uint64_t>(kmin, red64, [](uint64_t a, uint64_t b) { return a < b ? a : b; }, ~0ull);
   kmax = block_reduce<uint64_t>(kmax, red64, [](uint64_t a, uint64_t b) { return a > b ? a : b; }, 0ull);
 
-  // ---- threshold: count(key >= lo) in [n_res, n_res + kSelSlack] (keys are distinct, so it exists).
-  // Radix descent over the window [base, win_hi] of the key space that still holds the boundary: 256
-  // equal bins, a shared-memory histogram, a warp scan from the top bin down to the bin where the count
-  // crosses what is still needed; that bin becomes the next window.  Candidate keys cluster in a narrow
-  // score range, so the window is sized from (kmin, kmax) instead of the 64-bit digit positions: two or
-  // three levels where a bisection takes ~30 counting rounds.
+  // ---- threshold: count(key >= lo) in [n_res, n_res + kSelSlack] (keys are distinct, so it exists)
   uint64_t lo = kmin;
   if (total > n_res + kSelSlack) {
-    uint64_t base = kmin, win_hi = kmax;
-    int need = n_res;  // keys still to take from the window; everything above the window is taken
-    int shift = 64 - __clzll((long long)((kmax - kmin) | 1ull)) - 8;
-    shift = shift < 0 ? 0 : shift;
-    for (;;) {
-      for (int b = tid; b < 256; b += kSelThreads) hist[b] = 0;
-      __syncthreads();
-      for (int i = tid; i < total; i += kSelThreads) {
-        const uint64_t key = keys[i];
-        if (key >= base && key <= win_hi) atomicAdd(&hist[(int)((key - base) >> shift)], 1);
-      }
-      __syncthreads();
-      if (warp == 0) {
-        // lane l owns bins [8l, 8l + 8); suf = keys in the bins of lanes >= l
-        int own = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) own += hist[8 * lane + j];
-        int suf = own;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-          const int v = __shfl_down_sync(kFull, suf, off);
-          if (lane + off < 32) suf += v;
-        }
-        // the crossing lane: suf >= need while the lanes above it hold fewer than need
-        if (suf >= need && suf - own < need) {
-          int above = suf - own, b = 8 * lane + 7;
-          for (; b > 8 * lane; --b) {
-            if (above + hist[b] >= need) break;
-            above += hist[b];
-          }
-          sel_bin = b;
-          sel_above = above;
-        }
-      }
-      __syncthreads();
-      const int b = sel_bin, above = sel_above, in_bin = hist[b];
-      lo = base + ((uint64_t)b << shift);
-      if (above + in_bin <= need + kSelSlack || shift == 0) break;
-      need -= above;
-      base = lo;
-      win_hi = base + ((1ull << shift) - 1ull);
-      shift = shift > 8 ? shift - 8 : 0;
-      __syncthreads();  // hist / sel_bin are rewritten by the next level
-    }
+    const auto each_key = [&](auto f) {
+      for (int i = tid; i < total; i += kSelThreads) f(keys[i]);
+    };
+    lo = select_keys<kSelThreads>(each_key, kmin, kmax, n_res, kSelSlack, sel).lo;
   }
   // ---- collect the selected candidates
   for (int i = tid; i < total; i += kSelThreads) {
@@ -629,28 +571,13 @@ select_rescore_kernel(const uint2* __restrict__ cand, const int32_t* __restrict_
       }
     }
     __syncthreads();
-    // ---- rank by counting under (score desc, index asc); ranks are a permutation
+    // ---- rank under (score desc, index asc)
     for (int c = tid; c < ns; c += kSelThreads) {
-      const double sc = sel_score[c];
-      const uint32_t ic = sel_idx[c];
-      int rank = 0;
-      for (int j = 0; j < ns; ++j) {
-        const double sj = sel_score[j];
-        rank += (sj > sc || (sj == sc && sel_idx[j] < ic)) ? 1 : 0;
-      }
-      if (rank < k) {
-        const size_t oo = (size_t)q * k + rank;
-        o.scores[oo] = (float)sc;
-        if (o.scores64) o.scores64[oo] = sc;
-        o.idx[oo] = (int64_t)ic + o.idx_offset;
-        if (o.packed) {
-          o.packed[2 * oo] = __double_as_longlong(sc);
-          o.packed[2 * oo + 1] = (int64_t)ic + o.idx_offset;
-        }
-      }
+      const int rank = rank_desc(sel_score, sel_idx, ns, c);
+      if (rank < k) o.out.put(q, k, rank, sel_score[c], sel_idx[c]);
       if (rank == k - 1) {
-        kth_score = sc;
-        kth_idx = ic;
+        kth_score = sel_score[c];
+        kth_idx = sel_idx[c];
       }
     }
     __syncthreads();
@@ -681,20 +608,9 @@ select_rescore_kernel(const uint2* __restrict__ cand, const int32_t* __restrict_
     lo = lo2;
   }
 
-  const int valid = ns < k ? ns : k;
-  for (int r = valid + tid; r < k; r += kSelThreads) {
-    const size_t oo = (size_t)q * k + r;
-    o.scores[oo] = -INFINITY;
-    if (o.scores64) o.scores64[oo] = -INFINITY;
-    o.idx[oo] = -1;
-    if (o.packed) {
-      o.packed[2 * oo] = __double_as_longlong(-INFINITY);
-      o.packed[2 * oo + 1] = -1;
-    }
-  }
+  o.out.pad(q, k, ns < k ? ns : k, tid, kSelThreads);
   err = block_reduce<float>(err, redf, [](float a, float b) { return fmaxf(a, b); }, 0.f);
   if (tid == 0) {
-    if (o.count) o.count[q] = valid;
     atomicMax(&o.guard.state->max_err_bits, __float_as_uint(err));
     atomicMax(&o.guard.state->max_eps_bits, __float_as_uint(eps));
     if (!proven) guard_flag(o.guard, o.q_base + q, k, ns, kth_score, kth_idx);
@@ -707,8 +623,7 @@ select_rescore_kernel(const uint2* __restrict__ cand, const int32_t* __restrict_
 template <bool PACKED>
 __global__ void __launch_bounds__(256)
 topk_merge_kernel(const double* __restrict__ scores, const int64_t* __restrict__ idx, int n_parts, int nq, int k,
-                  float* __restrict__ out_scores, double* __restrict__ out_scores64, int64_t* __restrict__ out_idx,
-                  int32_t* __restrict__ out_count) {
+                  const TopkOut out) {
   extern __shared__ __align__(16) uint8_t sm_raw[];
   const int n = n_parts * k;
   double* s = reinterpret_cast<double*>(sm_raw);
@@ -755,21 +670,9 @@ topk_merge_kernel(const double* __restrict__ scores, const int64_t* __restrict__
       }
       rank += lo;
     }
-    if (rank < k) {
-      const size_t o = (size_t)q * k + rank;
-      out_scores[o] = (float)sc;
-      if (out_scores64) out_scores64[o] = sc;
-      out_idx[o] = ic;
-    }
+    if (rank < k) out.put(q, k, rank, sc, ic);
   }
-  const int valid = n_valid < k ? n_valid : k;
-  for (int r = valid + tid; r < k; r += blockDim.x) {
-    const size_t o = (size_t)q * k + r;
-    out_scores[o] = -INFINITY;
-    if (out_scores64) out_scores64[o] = -INFINITY;
-    out_idx[o] = -1;
-  }
-  if (out_count && tid == 0) out_count[q] = valid;
+  out.pad(q, k, n_valid < k ? n_valid : k, tid, blockDim.x);
 }
 
 struct SimPlan {
@@ -907,15 +810,8 @@ int run_mma_topk(const TopkCall& c, void* ws, size_t ws_bytes) {
       }
     }
     SelectOut so;
-    so.scores = c.out_scores + (size_t)q0 * k;
-    so.scores64 = c.out_scores64 ? c.out_scores64 + (size_t)q0 * k : nullptr;
-    so.idx = c.out_idx + (size_t)q0 * k;
-    so.count = c.out_count ? c.out_count + q0 : nullptr;
-    so.packed = c.out_packed ? c.out_packed + (size_t)q0 * k * 2 : nullptr;
-    so.idx_offset = c.idx_offset;
-    so.guard.state = c.state;
-    so.guard.flagged = c.flagged;
-    so.guard.bounds = c.bounds;
+    so.out = c.out.at(q0, k);
+    so.guard = c.guard;
     so.guard_coeff = guard_coeff_mma(d);
     so.q_base = q0;
     if (nq_c >= kSelThroughputMinQueries) {
@@ -944,12 +840,11 @@ int launch_topk_merge(const double* d_scores64, const int64_t* d_idx_or_packed, 
     RPX_CUDA_OK(cudaFuncSetAttribute(topk_merge_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     configured = dev.device;
   }
+  const TopkOut out{d_out_scores, d_out_scores64, d_out_idx, d_out_count, nullptr, 0};
   if (packed)
-    topk_merge_kernel<true><<<nq, 256, smem, st>>>(nullptr, d_idx_or_packed, n_parts, nq, k, d_out_scores, d_out_scores64,
-                                                   d_out_idx, d_out_count);
+    topk_merge_kernel<true><<<nq, 256, smem, st>>>(nullptr, d_idx_or_packed, n_parts, nq, k, out);
   else
-    topk_merge_kernel<false><<<nq, 256, smem, st>>>(d_scores64, d_idx_or_packed, n_parts, nq, k, d_out_scores,
-                                                    d_out_scores64, d_out_idx, d_out_count);
+    topk_merge_kernel<false><<<nq, 256, smem, st>>>(d_scores64, d_idx_or_packed, n_parts, nq, k, out);
   RPX_CUDA_OK(cudaGetLastError());
   return RPX_OK;
 }

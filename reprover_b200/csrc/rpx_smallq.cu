@@ -1,4 +1,4 @@
-// rpx_smallq.cu — similarity + top-k for 1..4 queries as ONE HBM-bound streaming kernel.
+// rpx_smallq.cu — similarity + top-k for 1 or 2 queries as ONE HBM-bound streaming kernel.
 //
 // This is the shape the reference's only production call has: `PremiseRetriever.retrieve`
 // (retrieval/model.py:338-375, called per proof state from prover/tactic_generator.py:286-292)
@@ -24,7 +24,6 @@
 // No sampling pass, no memsets, no second launch (the exact-path kernel that follows returns at once
 // unless the guard flagged a query).
 #include "rpx_common.cuh"
-#include "rpx_kernels.cuh"
 #include "rpx_topk_common.cuh"
 
 namespace rpx {
@@ -38,29 +37,18 @@ constexpr int kSqCtaKeep = 16;    // keys a CTA hands to the tail
 constexpr int kSqSelMax = 288;    // >= n_res + selection slack for k <= 200
 constexpr int kSqSelSlack = 16;
 
-struct SqCand {
-  uint64_t key64;  // dkey(fp64 score); 0 = empty slot
-  uint64_t idx;    // local row
-};
-
 struct SmallQParams {
   const __nv_bfloat16* Q;
   const __nv_bfloat16* E;
   int64_t n;
-  int d, k, n_res;
+  int d, k;
   const uint32_t* mask;
   int64_t mask_stride;
-  float* out_scores;
-  double* out_scores64;
-  int64_t* out_idx;
-  int32_t* out_count;
-  int64_t* out_packed;
-  int64_t idx_offset;
+  TopkOut out;
   GuardOut guard;
-  SqCand* cta_cand;    // [grid][NQ][kSqCtaKeep] exact (fp64 score, row) of each CTA's best rows
+  TopkCand* cta_cand;  // [grid][NQ][kSqCtaKeep] exact (fp64 score, row) of each CTA's best rows
   uint64_t* cta_thr;   // [grid][NQ] best key that CTA dropped (0: none)
   float guard_coeff;
-  int q_base;          // number of the first query of this launch within the call (guard records)
 };
 
 __device__ __forceinline__ float dot8_acc(const uint4& e, const uint4& q, float acc) {
@@ -96,7 +84,7 @@ struct WarpHeap {
   }
 };
 
-// NQ queries (1, 2 or 4), ITS = 16-byte chunks per lane per row (ceil(d / 256)).
+// NQ queries (1 or 2), ITS = 16-byte chunks per lane per row (ceil(d / 256)).
 template <int NQ, int ITS>
 __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQParams p) {
   extern __shared__ __align__(16) uint8_t sm_raw[];
@@ -199,13 +187,13 @@ __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQ
   for (int t = warp; t < NQ * kSqCtaKeep; t += kSqWarps) {
     const int q = t / kSqCtaKeep;
     const uint64_t key = ckeys[t];
-    SqCand c;
-    c.key64 = 0ull;
+    TopkCand c;
+    c.key = 0ull;
     c.idx = ~0ull;
     if (key != 0ull) {
       const uint32_t row = ckey_idx(key);
       const double s = dot64_canonical(reinterpret_cast<const __nv_bfloat16*>(sQ + (size_t)q * CH), p.E + (size_t)row * d, d, lane);
-      c.key64 = dkey(s);
+      c.key = dkey(s);
       c.idx = row;
       err = fmaxf(err, fabsf((float)(s - (double)ckey_score(key))));
     }
@@ -234,7 +222,7 @@ __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQ
   __shared__ uint64_t red64[32];
   __shared__ float redf[32];
   __shared__ int redi[32];
-  __shared__ int cslots[3];
+  __shared__ SelectSmem sel;
   __shared__ int n_sel;
   __shared__ double kth_score;
   __shared__ uint32_t kth_idx;
@@ -244,8 +232,8 @@ __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQ
     int valid = 0;
     for (int i = tid; i < G; i += kSqThreads) {
       const int cta = i / kSqCtaKeep, s = i - cta * kSqCtaKeep;
-      const SqCand* src = &p.cta_cand[((size_t)cta * NQ + q) * kSqCtaKeep + s];
-      const uint64_t key = __ldcg(&src->key64);
+      const TopkCand* src = &p.cta_cand[((size_t)cta * NQ + q) * kSqCtaKeep + s];
+      const uint64_t key = __ldcg(&src->key);
       k64[i] = key;
       ix[i] = (uint32_t)__ldcg(&src->idx);
       if (key != 0ull) {
@@ -258,33 +246,21 @@ __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQ
       const uint64_t t = __ldcg(&p.cta_thr[(size_t)c * NQ + q]);
       udrop = t > udrop ? t : udrop;
     }
-    if (tid < 3) cslots[tid] = 0;
     if (tid == 0) n_sel = 0;
     kmin = block_reduce<uint64_t>(kmin, red64, [](uint64_t a, uint64_t b) { return a < b ? a : b; }, ~0ull);
     kmax = block_reduce<uint64_t>(kmax, red64, [](uint64_t a, uint64_t b) { return a > b ? a : b; }, 0ull);
     udrop = block_reduce<uint64_t>(udrop, red64, [](uint64_t a, uint64_t b) { return a > b ? a : b; }, 0ull);
     const int total = block_reduce<int>(valid, redi, [](int a, int b) { return a + b; }, 0);
     const int k = p.k;
-    // threshold on the fp64 keys: count(key >= lo) in [k, k + slack] unless ties hold it higher
+    // threshold on the fp64 keys: count(key >= lo) in [k, k + slack] unless ties hold it higher (empty slots,
+    // key 0, lie below kmin)
     uint64_t lo = total > 0 ? kmin : 1ull;
-    int count_lo = total;
     if (total > k + kSqSelSlack) {
-      uint64_t hi = kmax;  // count(>= kmax) >= 1; the loop keeps count(>= lo) >= k
-      for (int iter = 0; count_lo > k + kSqSelSlack && hi - lo > 1; ++iter) {
-        const uint64_t mid = lo + (hi - lo) / 2;
-        int m = 0;
-        for (int i = tid; i < G; i += kSqThreads) m += k64[i] >= mid ? 1 : 0;
-        m = block_count(m, cslots, iter);
-        if (m >= k) {
-          lo = mid;
-          count_lo = m;
-        } else {
-          hi = mid;
-        }
-      }
+      const auto each_key = [&](auto f) {
+        for (int i = tid; i < G; i += kSqThreads) f(k64[i]);
+      };
+      lo = select_keys<kSqThreads>(each_key, kmin, kmax, k, kSqSelSlack, sel).lo;
     }
-    // more exact ties at the k-th score than the ranking buffer holds: let the exact path do it
-    const bool overflow = count_lo > kSqSelMax;
     for (int i = tid; i < G; i += kSqThreads) {
       const uint64_t key = k64[i];
       if (key != 0ull && key >= lo) {
@@ -302,60 +278,38 @@ __global__ void __launch_bounds__(kSqThreads, 1) smallq_topk_kernel(const SmallQ
       q2 = fmaf(v, v, q2);
     }
     q2 = block_reduce<float>(q2, redf, [](float a, float b) { return a + b; }, 0.f);  // (also orders n_sel / sel_*)
-    const int ns = n_sel < kSqSelMax ? n_sel : kSqSelMax;
-    // rank by counting under (score desc, index asc); ranks are a permutation
+    // more exact ties at the k-th score than the ranking buffer holds: let the exact path do it
+    const bool overflow = n_sel > kSqSelMax;
+    const int ns = overflow ? kSqSelMax : n_sel;
     for (int c = tid; c < ns; c += kSqThreads) {
-      const uint64_t kc = sel_key[c];
-      const uint32_t ic = sel_idx[c];
-      int rank = 0;
-      for (int j = 0; j < ns; ++j) {
-        const uint64_t kj = sel_key[j];
-        rank += (kj > kc || (kj == kc && sel_idx[j] < ic)) ? 1 : 0;
-      }
+      const int rank = rank_desc(sel_key, sel_idx, ns, c);
       if (rank < k) {
-        const double sc = undkey(kc);
-        const size_t o = (size_t)q * k + rank;
-        p.out_scores[o] = (float)sc;
-        if (p.out_scores64) p.out_scores64[o] = sc;
-        p.out_idx[o] = (int64_t)ic + p.idx_offset;
-        if (p.out_packed) {
-          p.out_packed[2 * o] = __double_as_longlong(sc);
-          p.out_packed[2 * o + 1] = (int64_t)ic + p.idx_offset;
-        }
+        const double sc = undkey(sel_key[c]);
+        p.out.put(q, k, rank, sc, sel_idx[c]);
         if (rank == k - 1) {
           kth_score = sc;
-          kth_idx = ic;
+          kth_idx = sel_idx[c];
         }
       }
     }
     const int nvalid = ns < k ? ns : k;
-    for (int r = nvalid + tid; r < k; r += kSqThreads) {
-      const size_t o = (size_t)q * k + r;
-      p.out_scores[o] = -INFINITY;
-      if (p.out_scores64) p.out_scores64[o] = -INFINITY;
-      p.out_idx[o] = -1;
-      if (p.out_packed) {
-        p.out_packed[2 * o] = __double_as_longlong(-INFINITY);
-        p.out_packed[2 * o + 1] = -1;
-      }
-    }
+    p.out.pad(q, k, nvalid, tid, kSqThreads);
     __syncthreads();
     if (tid == 0) {
-      if (p.out_count) p.out_count[q] = nvalid;
       // the candidates were ranked by their exact scores; what can still be missing is a row a warp or
       // CTA heap dropped on its fp32 score (udrop = the best such key)
       const float u = udrop != 0ull ? ckey_score(udrop) : -INFINITY;
-      guard_decide(p.guard, p.q_base + q, k, overflow ? 0 : ns, kth_score, kth_idx, overflow ? INFINITY : u, q2,
-                   p.guard_coeff, 0.f);
+      guard_decide(p.guard, q, k, overflow ? 0 : ns, kth_score, kth_idx, overflow ? INFINITY : u, q2, p.guard_coeff,
+                   0.f);
     }
     __syncthreads();
   }
 }
 
-size_t smallq_smem_bytes(int nq_t, int d, int grid) {
+size_t smallq_smem_bytes(int nq, int d, int grid) {
   const size_t CH = (size_t)d >> 3;
-  size_t b = (size_t)nq_t * CH * 16;
-  b += (size_t)nq_t * (kSqWarps * kSqWarpKeep + kSqCtaKeep + 1) * 8;
+  size_t b = (size_t)nq * CH * 16;
+  b += (size_t)nq * (kSqWarps * kSqWarpKeep + kSqCtaKeep + 1) * 8;
   b += 16 + (size_t)grid * kSqCtaKeep * (8 + 4);           // tail: fp64 keys + rows
   b += 16 + (size_t)kSqSelMax * (8 + 4);                    // tail: ranking buffer
   return b;
@@ -385,56 +339,36 @@ int launch_its(const SmallQParams& p, int its, int grid, size_t smem, cudaStream
 
 }  // namespace
 
-bool smallq_supported(int nq, int k, int d) { return nq >= 1 && nq <= 4 && k >= 1 && k <= 200 && d % 8 == 0 && d <= 2048; }
+bool smallq_supported(int nq, int k, int d) { return nq >= 1 && nq <= 2 && k >= 1 && k <= 200 && d % 8 == 0 && d <= 2048; }
 
 size_t smallq_workspace_bytes(int num_sms) {
-  return align_up((size_t)num_sms * 4 * kSqCtaKeep * sizeof(SqCand), 256) + align_up((size_t)num_sms * 4 * 8, 256);
+  return align_up((size_t)num_sms * 2 * kSqCtaKeep * sizeof(TopkCand), 256) + align_up((size_t)num_sms * 2 * 8, 256);
 }
 
-// nq in 1..4: the kernel is instantiated for 1, 2 and 4 queries; 3 queries run as 2 + 1.
-int launch_smallq_topk(const TopkCall& c, void* ws, int n_res) {
+// one launch, instantiated for NQ = nq
+int launch_smallq_topk(const TopkCall& c, void* ws) {
   RPX_REQUIRE(smallq_supported(c.nq, c.k, c.d), RPX_ERR_UNSUPPORTED, "small-Q top-k: nq=%d k=%d d=%d", c.nq, c.k, c.d);
   DeviceInfo dev;
   RPX_TRY(get_device_info(&dev));
   const int grid = dev.num_sms;
   const int its = ((c.d >> 3) + 31) >> 5;
   uint8_t* base = static_cast<uint8_t*>(ws);
-  int q0 = 0;
-  while (q0 < c.nq) {
-    const int rest = c.nq - q0;
-    const int nq_t = rest >= 4 ? 4 : (rest >= 2 ? 2 : 1);
-    SmallQParams p;
-    p.Q = c.Q + (size_t)q0 * c.d;
-    p.E = c.E;
-    p.n = c.n;
-    p.d = c.d;
-    p.k = c.k;
-    p.n_res = n_res;
-    p.mask = c.mask ? c.mask + (size_t)q0 * c.mask_stride : nullptr;
-    p.mask_stride = c.mask_stride;
-    p.out_scores = c.out_scores + (size_t)q0 * c.k;
-    p.out_scores64 = c.out_scores64 ? c.out_scores64 + (size_t)q0 * c.k : nullptr;
-    p.out_idx = c.out_idx + (size_t)q0 * c.k;
-    p.out_count = c.out_count ? c.out_count + q0 : nullptr;
-    p.out_packed = c.out_packed ? c.out_packed + (size_t)q0 * c.k * 2 : nullptr;
-    p.idx_offset = c.idx_offset;
-    p.guard.state = c.state;
-    p.guard.flagged = c.flagged;
-    p.guard.bounds = c.bounds;
-    p.cta_cand = reinterpret_cast<SqCand*>(base);
-    p.cta_thr = reinterpret_cast<uint64_t*>(base + align_up((size_t)grid * 4 * kSqCtaKeep * sizeof(SqCand), 256));
-    p.guard_coeff = guard_coeff_stream(c.d);
-    p.q_base = q0;
-    const size_t smem = smallq_smem_bytes(nq_t, c.d, grid);
-    RPX_REQUIRE(smem <= 160 * 1024, RPX_ERR_UNSUPPORTED, "small-Q top-k: %zu B of shared memory", smem);
-    int rc;
-    if (nq_t == 4) rc = launch_its<4>(p, its, grid, smem, c.st, dev.device);
-    else if (nq_t == 2) rc = launch_its<2>(p, its, grid, smem, c.st, dev.device);
-    else rc = launch_its<1>(p, its, grid, smem, c.st, dev.device);
-    RPX_TRY(rc);
-    q0 += nq_t;
-  }
-  return RPX_OK;
+  SmallQParams p;
+  p.Q = c.Q;
+  p.E = c.E;
+  p.n = c.n;
+  p.d = c.d;
+  p.k = c.k;
+  p.mask = c.mask;
+  p.mask_stride = c.mask_stride;
+  p.out = c.out;
+  p.guard = c.guard;
+  p.cta_cand = reinterpret_cast<TopkCand*>(base);
+  p.cta_thr = reinterpret_cast<uint64_t*>(base + align_up((size_t)grid * 2 * kSqCtaKeep * sizeof(TopkCand), 256));
+  p.guard_coeff = guard_coeff_stream(c.d);
+  const size_t smem = smallq_smem_bytes(c.nq, c.d, grid);
+  RPX_REQUIRE(smem <= 160 * 1024, RPX_ERR_UNSUPPORTED, "small-Q top-k: %zu B of shared memory", smem);
+  return c.nq == 2 ? launch_its<2>(p, its, grid, smem, c.st, dev.device) : launch_its<1>(p, its, grid, smem, c.st, dev.device);
 }
 
 }  // namespace rpx

@@ -1,6 +1,7 @@
-// rpx_topk_common.cuh — device helpers shared by the three top-k paths
-// (rpx_simtopk.cu: tensor-core path, rpx_smallq.cu: HBM-streaming path for <= 4 queries,
-//  rpx_exact.cu: exact fp64 fallback) and the device-resident state of an index handle.
+// rpx_topk_common.cuh — what the top-k kernels share (rpx_simtopk.cu: tensor-core path, rpx_smallq.cu:
+// HBM-streaming path for 1-2 queries, rpx_exact.cu: exact fp64 fallback, rpx_bm25.cu: BM25 tiles) and their
+// host-side entry points: the device-resident state of an index handle, the result writer, the key selection
+// and the ranking every kernel ends with, and the exactness guard.
 //
 // Ordering contract (include/rpx.h): score descending, then index ascending, where score is the
 // canonical fp64 dot product of the bf16 operands (dot64_canonical == oracle/rpx_oracle.c::
@@ -11,6 +12,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace rpx {
@@ -78,17 +80,142 @@ __device__ __forceinline__ T block_reduce(T v, T* red, Op op, T identity) {
   return r;
 }
 
-// Block-wide sum of per-thread counts with ONE barrier per call: warp REDUX, one shared-memory
-// atomic per warp, three rotating counters (slot i % 3 is used by call i and cleared during call
-// i + 1, well before call i + 3 adds to it again).  `slots` must be zero on the first call.
-__device__ __forceinline__ int block_count(int m, int* slots, int iter) {
-  m = __reduce_add_sync(kFullMask, m);
-  int* cur = slots + iter % 3;
-  if ((threadIdx.x & 31) == 0 && m != 0) atomicAdd(cur, m);
-  __syncthreads();
-  const int total = *cur;
-  if (threadIdx.x == 0) slots[(iter + 2) % 3] = 0;
-  return total;
+// One selected candidate: dkey(fp64 score) and local row.
+struct TopkCand {
+  uint64_t key;  // 0 = empty slot
+  uint64_t idx;
+};
+
+// Where a call's results go: k entries per query, ranked under the contract; ranks past the valid entries
+// hold (-inf, -1).  All pointers are device pointers.
+struct TopkOut {
+  float* scores;        // [nq, k]  (null: not written)
+  double* scores64;     // optional [nq, k]
+  int64_t* idx;         // [nq, k]
+  int32_t* count;       // optional [nq]: valid entries
+  int64_t* packed;      // optional [nq, k, 2]: (fp64 score bits, index) — the all-gather payload
+  int64_t idx_offset;   // added to every local row written
+
+  __device__ __forceinline__ void put(int q, int k, int rank, double score, int64_t row) const {
+    const size_t o = (size_t)q * k + rank;
+    if (scores) scores[o] = (float)score;
+    if (scores64) scores64[o] = score;
+    idx[o] = row + idx_offset;
+    if (packed) {
+      packed[2 * o] = __double_as_longlong(score);
+      packed[2 * o + 1] = row + idx_offset;
+    }
+  }
+  // ranks [valid, k) of query q; thread `tid` of `nthreads` writes every nthreads-th of them, tid 0 the count
+  __device__ __forceinline__ void pad(int q, int k, int valid, int tid, int nthreads) const {
+    for (int r = valid + tid; r < k; r += nthreads) {
+      const size_t o = (size_t)q * k + r;
+      if (scores) scores[o] = -INFINITY;
+      if (scores64) scores64[o] = -INFINITY;
+      idx[o] = -1;
+      if (packed) {
+        packed[2 * o] = __double_as_longlong(-INFINITY);
+        packed[2 * o + 1] = -1;
+      }
+    }
+    if (count && tid == 0) count[q] = valid;
+  }
+  // the results of queries q0, q0 + 1, ...
+  TopkOut at(int q0, int k) const {
+    TopkOut o = *this;
+    const size_t off = (size_t)q0 * k;
+    o.scores = scores ? scores + off : nullptr;
+    o.scores64 = scores64 ? scores64 + off : nullptr;
+    o.idx = idx + off;
+    o.count = count ? count + q0 : nullptr;
+    o.packed = packed ? packed + 2 * off : nullptr;
+    return o;
+  }
+};
+
+// Rank of entry c among keys[0, n) under (key desc, idx asc), by counting.  Over distinct (key, idx) pairs
+// the ranks are a permutation of 0..n-1.
+template <typename K, typename I>
+__device__ __forceinline__ int rank_desc(const K* keys, const I* idx, int n, int c) {
+  const K kc = keys[c];
+  const I ic = idx[c];
+  int rank = 0;
+  for (int j = 0; j < n; ++j) {
+    const K kj = keys[j];
+    rank += (kj > kc || (kj == kc && idx[j] < ic)) ? 1 : 0;
+  }
+  return rank;
+}
+
+struct SelectSmem {
+  int hist[256];
+  int bin, above;
+};
+
+struct KeyCut {
+  uint64_t lo;   // every key >= lo is selected (n_above >= 0: every key > lo and need - n_above keys == lo)
+  int n_above;   // -1, or the window narrowed to single key values: count(key > lo), lo is the need-th key
+};
+
+// Block-wide selection of the `need` largest of a set of 64-bit keys (need <= set size), called by all
+// kThreads threads.  `for_each_key(f)` calls f(key) on the keys this thread holds, wherever they sit (shared
+// memory, global memory, registers); every key lies in [kmin, kmax].  Returns lo with
+// need <= count(key >= lo) <= need + slack, or, when ties at the need-th key hold that count higher, that key
+// itself with n_above = count(key > lo).
+// Radix descent over the window [base, win_hi] of the key space that still holds the boundary: 256 equal
+// bins, a shared-memory histogram, warp 0 finds the bin where the count from the top crosses what is still
+// needed; that bin becomes the next window.  The window is sized from (kmin, kmax), not from the digit
+// positions, so keys that cluster in a narrow range take two or three levels.  `sm` is read until the call
+// returns: a barrier must separate the call from the next write to it.
+template <int kThreads, class ForEachKey>
+__device__ __forceinline__ KeyCut select_keys(ForEachKey for_each_key, uint64_t kmin, uint64_t kmax, int need,
+                                              int slack, SelectSmem& sm) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int taken = 0;  // keys above the window, all selected
+  uint64_t base = kmin, win_hi = kmax;
+  int shift = 64 - __clzll((long long)((kmax - kmin) | 1ull)) - 8;
+  shift = shift < 0 ? 0 : shift;
+  for (;;) {
+    for (int b = tid; b < 256; b += kThreads) sm.hist[b] = 0;
+    __syncthreads();
+    for_each_key([&](uint64_t key) {
+      if (key >= base && key <= win_hi) atomicAdd(&sm.hist[(int)((key - base) >> shift)], 1);
+    });
+    __syncthreads();
+    if (warp == 0) {
+      // lane l owns bins [8l, 8l + 8); suf = keys in the bins of lanes >= l
+      int own = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) own += sm.hist[8 * lane + j];
+      int suf = own;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int v = __shfl_down_sync(kFullMask, suf, off);
+        if (lane + off < 32) suf += v;
+      }
+      // the crossing lane: suf >= need while the lanes above it hold fewer than need
+      if (suf >= need && suf - own < need) {
+        int above = suf - own, b = 8 * lane + 7;
+        for (; b > 8 * lane; --b) {
+          if (above + sm.hist[b] >= need) break;
+          above += sm.hist[b];
+        }
+        sm.bin = b;
+        sm.above = above;
+      }
+    }
+    __syncthreads();
+    const int b = sm.bin, above = sm.above, in_bin = sm.hist[b];
+    const uint64_t lo = base + ((uint64_t)b << shift);
+    if (above + in_bin <= need + slack) return KeyCut{lo, -1};
+    if (shift == 0) return KeyCut{lo, taken + above};
+    need -= above;
+    taken += above;
+    base = lo;
+    win_hi = base + ((1ull << shift) - 1ull);
+    shift = shift > 8 ? shift - 8 : 0;
+    __syncthreads();  // hist / bin are rewritten by the next level
+  }
 }
 
 // Canonical fp64 dot product (identical in oracle/rpx_oracle.c::rpx_oracle_dot64):
@@ -213,5 +340,36 @@ __device__ __forceinline__ bool guard_decide(const GuardOut& g, int q, int k, in
   if (!proven) guard_flag(g, q, k, n_ranked, kth_score, kth_idx);
   return proven;
 }
+
+// ------------------------------------------------------------------------------- host entry points
+// One similarity + top-k request (all pointers are device pointers).
+struct TopkCall {
+  const __nv_bfloat16* Q;   // [nq, d]
+  int nq;
+  const __nv_bfloat16* E;   // [n, d]
+  int64_t n;
+  int d, k;
+  const uint32_t* mask;     // optional access bitmask [nq][mask_stride]
+  int64_t mask_stride;
+  TopkOut out;
+  GuardOut guard;           // state of the index handle, [nq] guard scratch
+  cudaStream_t st;
+};
+// re-score set size for k results (k + margin; the guard covers what the margin does not)
+inline int topk_n_res(int k) { return k + (k / 8 > 12 ? k / 8 : 12); }
+constexpr int kFastPathMaxK = 200;   // larger k goes through the exact path
+
+int launch_row_norm_max(const __nv_bfloat16* E, int64_t n, int d, IndexState* state, cudaStream_t st);
+size_t exact_cand_bytes(int64_t n);
+int launch_exact_topk(const TopkCall& c, void* cand_ws, bool all_queries);
+bool smallq_supported(int nq, int k, int d);
+size_t smallq_workspace_bytes(int num_sms);
+int launch_smallq_topk(const TopkCall& c, void* ws);
+size_t mma_topk_workspace_bytes(int nq, int k, int d, int num_sms);
+int run_mma_topk(const TopkCall& c, void* ws, size_t ws_bytes);
+// k-way merge of per-shard results; `packed`: one [n_parts, nq, k, 2] (score bits, index) buffer.
+int launch_topk_merge(const double* d_scores64, const int64_t* d_idx_or_packed, bool packed, int n_parts, int nq, int k,
+                      float* d_out_scores, double* d_out_scores64, int64_t* d_out_idx, int32_t* d_out_count,
+                      cudaStream_t st);
 
 }  // namespace rpx

@@ -37,7 +37,7 @@ for nq in [int(x) for x in args.queries.split(",")]:
         words = np.packbits(m.reshape(nq, -1, 8), axis=2, bitorder="little").reshape(nq, -1).view("<u4").copy()
         mask = torch.from_numpy(words.view(np.int32)).to(dev)
     for name, flags in (("auto", 0), ("mma", _native.RPX_TOPK_FORCE_MMA), ("stream", _native.RPX_TOPK_FORCE_STREAM)):
-        if name == "stream" and nq > 4:
+        if name == "stream" and nq > 2:
             continue
         for _ in range(5):
             sim_topk(Q, h, args.k, access_mask=mask, flags=flags)
