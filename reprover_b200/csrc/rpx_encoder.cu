@@ -27,12 +27,6 @@ namespace rpx {
 
 namespace {
 
-// Throughput-path tiles of QKV: 128 x 128.  The accumulator tile (64 KB) and a 4-deep operand ring fit the 227 KB
-// of shared memory an H100 block may use.  The gated FFN up-projection, O-proj and FFN-down run on
-// gemm_ws_kernel's 128 x 256 tiles instead (rpx_gemm_ws.cuh); QKV measured 6 % slower there, its epilogue no
-// longer overlapping the next tile's MMAs.
-constexpr int kBlockN = 128;
-
 struct LayerW {
   const __nv_bfloat16* qkv;  // [3*inner, D]   (ln0 folded)
   const __nv_bfloat16* o;    // [D, inner]
@@ -274,10 +268,21 @@ int ss_parts(int d_model, bool latency) { return ceil_div(d_model, latency ? 32 
 // epilogue tests run exactly the launches an encode call runs.  A is [T, K], B is [N, K] (packed weights).
 
 // out [T, N] = bf16(A B^T * rs[m]).  On the latency path the CTAs the GEMM leaves idle fetch `prefetch` into L2.
+// The throughput path runs gemm_ws_kernel as pairs with a 4-stage ring: for ByT5-small (N = 1152) four full n-tiles
+// and one whose MMAs are 128 columns wide.  At 2^18 tokens on an H100 80GB HBM3 at a 700 W power limit (SM clock
+// 1980 MHz, tools/encoder_gemm_bench.py, three alternated runs of each form, the epilogue still storing 4 bytes
+// per lane) it took:
+//   4 stages, pairs        1.652-1.666 ms
+//   3 stages, pairs        1.666-1.673 ms
+//   4 stages, unclustered  1.831-1.835 ms
+//   3 stages, unclustered  1.800-1.819 ms
+//   gemm_tc_kernel, 128 x 128 tiles, 4 stages  1.723-1.741 ms
+// With the epilogue's 16-byte stores (quad_columns) the chosen form took 1.430-1.474 ms against 1.748-1.775 ms
+// for gemm_tc_kernel in the same alternated runs.
 int qkv_gemm(bool latency, int T, const void* A, const void* B, int N, int K, const RowScale& rs, __nv_bfloat16* out,
              const void* prefetch, size_t prefetch_bytes, cudaStream_t st) {
   EpiStoreBF16::Params ep{out, N, rs};
-  if (!latency) return launch_gemm<kBlockN, EpiStoreBF16>(A, K, B, K, T, N, K, ep, st);
+  if (!latency) return launch_gemm_ws<EpiWsStoreBF16, 4, 2>(A, K, B, K, T, N, K, ep, st);
   if (T <= kLatSmallMMaxTokens)
     return launch_gemm<kLatBlockN, EpiStoreBF16, false, kLatSmallStages, false, kLatSmallM>(A, K, B, K, T, N, K, ep, st,
                                                                                              prefetch, prefetch_bytes);

@@ -402,7 +402,8 @@ struct EpiStoreF32 {
   __device__ void finish() {}
 };
 
-// C[m, n] = bf16(acc * rs[m]).  QKV projection (RMSNorm folded: prologue of K3).
+// C[m, n] = bf16(acc * rs[m]).  QKV projection (RMSNorm folded: prologue of K3) of the latency path.  The
+// throughput path runs EpiWsStoreBF16 (rpx_gemm_ws.cuh).
 struct EpiStoreBF16 {
   struct Params {
     __nv_bfloat16* C;

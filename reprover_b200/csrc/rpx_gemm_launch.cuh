@@ -1,5 +1,6 @@
 // rpx_gemm_launch.cuh — the host-side launchers of the two contraction cores: launch_gemm (gemm_tc_kernel, for the
-// encoder's QKV and latency-path GEMMs and the similarity stages) and launch_gemm_ws (gemm_ws_kernel).
+// encoder's latency-path GEMMs and the similarity stages) and launch_gemm_ws (gemm_ws_kernel, for the encoder's
+// throughput-path GEMMs).
 #pragma once
 #include "rpx_common.cuh"
 #include "rpx_gemm.cuh"

@@ -19,6 +19,11 @@
 //                     the producer (`empty[]`) once the wgmma group that read it has retired: lane 0 of each
 //                     consumer warp arrives once for its warp.  After the last k-block each consumer runs the
 //                     epilogue functor on its own fragment.
+//                     The last n-tile of an N that is not a multiple of 256 runs its k-loop on m64nWk16 with W its
+//                     column count rounded up to 64 (the accumulator prefix acc[0, W/2)), chosen once per tile:
+//                     the B rows past N are still loaded as TMA zero-fill, but only those below W reach the
+//                     tensor cores.  The order of the additions over k, and so every output bit, is that of the
+//                     full-width MMA.
 //
 // CLUSTER = 2: the CTAs run as clusters of two on vertically adjacent tiles.  A work unit is an (m-tile pair,
 // n-tile), units visited n-fastest; rank r of the cluster takes m-tile 2 (u / tiles_n) + r.  Both need the same
@@ -44,6 +49,8 @@
 // acc[4j+2], acc[4j+3] the same columns of row r0 + 8, for j = 0..31.  A quad of lanes holds 8 contiguous
 // columns of a row: fp32 accesses from the fragment fill whole 32-byte sectors.
 #pragma once
+#include <type_traits>
+
 #include "rpx_gemm.cuh"
 
 namespace rpx {
@@ -83,6 +90,16 @@ struct ResStream {
   uint64_t* full;   // kResBufs mbarriers: the producer's TMA landed
   uint64_t* empty;  // kResBufs mbarriers: all 128 consumer threads are done with the buffer
 };
+
+// wgmma.m64nWk16 on the first W/2 registers of a consumer's accumulator (rpx_ptx.cuh).
+template <int W>
+RPX_DEVICE void wgmma_ws(float (&acc)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  static_assert(W == 64 || W == 128 || W == 192 || W == 256, "MMA width: a multiple of 64 up to the tile width");
+  if constexpr (W == 64) wgmma_m64n64k16_ss(acc, desc_a, desc_b, accumulate);
+  else if constexpr (W == 128) wgmma_m64n128k16_ss(acc, desc_a, desc_b, accumulate);
+  else if constexpr (W == 192) wgmma_m64n192k16_ss(acc, desc_a, desc_b, accumulate);
+  else wgmma_m64n256k16_ss(acc, desc_a, desc_b, accumulate);
+}
 
 // Epi must provide:
 //   struct Params;                                  (trivially copyable kernel argument)
@@ -214,16 +231,10 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (CLUSTER > 1) mbar_arrive_cluster(&empty[st], (uint32_t)(rank ^ 1));
       }
     };
-    for (int u = u0; u < num_units; u += u_step) {
-      FragCtx c;
-      c.n_blk = u % tiles_n;
-      c.m0 = unit_m(u) * kBlockM;
-      c.n0 = c.n_blk * kWsBlockN;
-      c.n_cols = N - c.n0 < kWsBlockN ? N - c.n0 : kWsBlockN;
-      c.M = M;
-      c.N = N;
-      c.r0 = c.m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2);
-      c.q = lane & 3;
+    // One tile's k-loop on MMAs W columns wide (W a compile-time constant: no branch between wgmma forms
+    // inside the loop).
+    auto mainloop = [&](auto width, const FragCtx& c) {
+      constexpr int W = decltype(width)::value;
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
@@ -233,7 +244,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         wgmma_fence_operand(acc);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / kMmaK; ++k) wgmma_m64n256k16_ss(acc, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
+        for (int k = 0; k < kBlockK / kMmaK; ++k) wgmma_ws<W>(acc, a_desc + 2 * k, b_desc + 2 * k, (kb | k) != 0);
         wgmma_commit();
         if (kb == 0) epi.prefetch(c);
         // the group of the previous k-block has retired once at most this one is in flight: its stage is free
@@ -250,6 +261,25 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_wait<0>();
       wgmma_fence_operand(acc);
       release(prev);
+    };
+    for (int u = u0; u < num_units; u += u_step) {
+      FragCtx c;
+      c.n_blk = u % tiles_n;
+      c.m0 = unit_m(u) * kBlockM;
+      c.n0 = c.n_blk * kWsBlockN;
+      c.n_cols = N - c.n0 < kWsBlockN ? N - c.n0 : kWsBlockN;
+      c.M = M;
+      c.N = N;
+      c.r0 = c.m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2);
+      c.q = lane & 3;
+      // The last n-tile of an N that is not a multiple of 256 issues MMAs only as wide as its columns rounded up
+      // to 64; the B rows between n_cols and that width are TMA zero-fill, as are those past it, which no MMA reads.
+      switch ((c.n_cols + 63) / 64) {
+        case 1: mainloop(std::integral_constant<int, 64>{}, c); break;
+        case 2: mainloop(std::integral_constant<int, 128>{}, c); break;
+        case 3: mainloop(std::integral_constant<int, 192>{}, c); break;
+        default: mainloop(std::integral_constant<int, 256>{}, c); break;
+      }
       epi.tile(c, acc);
     }
   }
@@ -261,7 +291,38 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 }
 
 // ============================================================================ register-fragment epilogues
-// Same arithmetic as EpiStoreF32 / EpiGeGLUT of rpx_gemm.cuh, element for element.
+// Same arithmetic as EpiStoreF32 / EpiStoreBF16 / EpiGeGLUT of rpx_gemm.cuh, element for element.
+
+// bf16 stores of a quad's fragment as 16-byte vectors.  Lane q of a quad holds, for a row and a block of 32
+// columns, the bf16 pairs x_t at columns 8t + 2q, 8t + 2q + 1 (t = 0..3, fragment blocks j = 4b + t); the four
+// lanes exchange them (a 4 x 4 transpose, two xor shuffles per stage) so that lane q returns columns
+// [8q, 8q + 8) of the block.  A warp then stores 64 contiguous bytes per row and instruction instead of 16.
+// Every lane of the warp must call it.
+RPX_DEVICE uint4 quad_columns(uint32_t x0, uint32_t x1, uint32_t x2, uint32_t x3, int q) {
+  // stage 1 (lanes q, q ^ 2): the off-diagonal 2 x 2 blocks
+  const bool hi = q & 2;
+  uint32_t r0 = __shfl_xor_sync(0xffffffffu, hi ? x0 : x2, 2);
+  uint32_t r1 = __shfl_xor_sync(0xffffffffu, hi ? x1 : x3, 2);
+  if (hi) {
+    x0 = r0;
+    x1 = r1;
+  } else {
+    x2 = r0;
+    x3 = r1;
+  }
+  // stage 2 (lanes q, q ^ 1): inside each 2 x 2 block
+  const bool odd = q & 1;
+  r0 = __shfl_xor_sync(0xffffffffu, odd ? x0 : x1, 1);
+  r1 = __shfl_xor_sync(0xffffffffu, odd ? x2 : x3, 1);
+  if (odd) {
+    x0 = r0;
+    x2 = r1;
+  } else {
+    x1 = r0;
+    x3 = r1;
+  }
+  return make_uint4(x0, x1, x2, x3);
+}
 
 // C[m, n] = acc (fp32).  The bare core behind rpx_gemm_bf16_f32.
 struct EpiWsStoreF32 {
@@ -277,6 +338,34 @@ struct EpiWsStoreF32 {
         float* dst = p.C + (size_t)c.r0 * p.ldc + c.n0 + 8 * j + 2 * c.q;
         if (c.r0 < c.M) *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j], acc[4 * j + 1]);
         if (c.r0 + 8 < c.M) *reinterpret_cast<float2*>(dst + 8 * (size_t)p.ldc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+    }
+  }
+};
+
+// C[m, n] = bf16(acc * rs[m]).  The QKV projection (RMSNorm folded: the weight into B, the row scale here).
+struct EpiWsStoreBF16 {
+  using Params = EpiStoreBF16::Params;
+  static constexpr int kResBufs = 0;
+  Params p;
+  float rs0 = 0.f, rs1 = 0.f;
+  __device__ EpiWsStoreBF16(const Params& p_, const ResStream&) : p(p_) {}
+  __device__ void prefetch(const FragCtx& c) {
+    rs0 = c.r0 < c.M ? p.rs.get(c.r0) : 0.f;
+    rs1 = c.r0 + 8 < c.M ? p.rs.get(c.r0 + 8) : 0.f;
+  }
+  __device__ void tile(const FragCtx& c, const float (&acc)[128]) {
+    __nv_bfloat16* dst = p.C + (size_t)c.r0 * p.ldc + c.n0 + 8 * c.q;
+#pragma unroll
+    for (int b = 0; b < 8; ++b) {  // 32-column blocks (n_cols is a multiple of 32: a block is valid or not, warp-wide)
+      if (32 * b < c.n_cols) {
+        const float* a = acc + 16 * b;
+        const uint4 v0 = quad_columns(pack_bf16x2(a[0] * rs0, a[1] * rs0), pack_bf16x2(a[4] * rs0, a[5] * rs0),
+                                      pack_bf16x2(a[8] * rs0, a[9] * rs0), pack_bf16x2(a[12] * rs0, a[13] * rs0), c.q);
+        const uint4 v1 = quad_columns(pack_bf16x2(a[2] * rs1, a[3] * rs1), pack_bf16x2(a[6] * rs1, a[7] * rs1),
+                                      pack_bf16x2(a[10] * rs1, a[11] * rs1), pack_bf16x2(a[14] * rs1, a[15] * rs1), c.q);
+        if (c.r0 < c.M) *reinterpret_cast<uint4*>(dst + 32 * b) = v0;
+        if (c.r0 + 8 < c.M) *reinterpret_cast<uint4*>(dst + 8 * (size_t)p.ldc + 32 * b) = v1;
       }
     }
   }
@@ -301,17 +390,21 @@ struct EpiWsGeGLU {
     rs1 = c.r0 + 8 < c.M ? p.rs.get(c.r0 + 8) : 0.f;
   }
   __device__ void tile(const FragCtx& c, const float (&acc)[128]) {
-    __nv_bfloat16* dst = p.out + (size_t)c.r0 * p.ldo + c.n_blk * (kWsBlockN / 2) + 2 * c.q;
+    __nv_bfloat16* dst = p.out + (size_t)c.r0 * p.ldo + c.n_blk * (kWsBlockN / 2) + 8 * c.q;
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const float* g = acc + 4 * j;
-      const float* u = acc + 4 * (j + 16);
-      if (c.r0 < c.M)
-        *reinterpret_cast<uint32_t*>(dst + 8 * j) =
-            pack_bf16x2(gelu_new(g[0] * rs0) * (u[0] * rs0), gelu_new(g[1] * rs0) * (u[1] * rs0));
-      if (c.r0 + 8 < c.M)
-        *reinterpret_cast<uint32_t*>(dst + 8 * (size_t)p.ldo + 8 * j) =
-            pack_bf16x2(gelu_new(g[2] * rs1) * (u[2] * rs1), gelu_new(g[3] * rs1) * (u[3] * rs1));
+    for (int b = 0; b < 4; ++b) {  // 32-column blocks of the output
+      uint32_t w0[4], w1[4];
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        const float* g = acc + 4 * (4 * b + t);
+        const float* u = acc + 4 * (4 * b + t + 16);
+        w0[t] = pack_bf16x2(gelu_new(g[0] * rs0) * (u[0] * rs0), gelu_new(g[1] * rs0) * (u[1] * rs0));
+        w1[t] = pack_bf16x2(gelu_new(g[2] * rs1) * (u[2] * rs1), gelu_new(g[3] * rs1) * (u[3] * rs1));
+      }
+      const uint4 v0 = quad_columns(w0[0], w0[1], w0[2], w0[3], c.q);
+      const uint4 v1 = quad_columns(w1[0], w1[1], w1[2], w1[3], c.q);
+      if (c.r0 < c.M) *reinterpret_cast<uint4*>(dst + 32 * b) = v0;
+      if (c.r0 + 8 < c.M) *reinterpret_cast<uint4*>(dst + 8 * (size_t)p.ldo + 32 * b) = v1;
     }
   }
 };
