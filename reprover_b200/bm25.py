@@ -274,26 +274,29 @@ def okapi_postings(documents: Sequence[Sequence[int]], vocab_size: Optional[int]
     return st
 
 
-def load_theorems(data_path: str) -> List[Dict[str, Any]]:
-    """The theorems of `train.json`, `val.json` and `test.json` under `data_path`, in that order (main.py:124-129)."""
+def load_theorems(data_path: str, splits: Sequence[str] = ("train", "val", "test")) -> List[Dict[str, Any]]:
+    """The theorems of `<split>.json` under `data_path` for each split, in that order (by default train, val and
+    test, as main.py:124-129 reads them)."""
     import json
     import os
 
     theorems: List[Dict[str, Any]] = []
-    for split in ("train", "val", "test"):
+    for split in splits:
         with open(os.path.join(data_path, f"{split}.json")) as fh:
             theorems.extend(json.load(fh))
     return theorems
 
 
 def all_pos_premises(annotated_tactic: Any, corpus: Corpus) -> list:
-    """Premises used by an annotated tactic that the corpus can locate (reference common.py:341-354)."""
+    """Premises used by an annotated tactic that the corpus can locate (reference common.py:341-354): each one once,
+    in the order of its first provenance.  The reference returns the same set as `list(set)`, whose order varies
+    with the process's string hashing; a fixed order makes prediction files reproducible byte for byte."""
     _, provenances = annotated_tactic
-    found = set()
+    found = {}
     for prov in provenances:
         p = corpus.locate_premise(prov["def_path"], Pos(*prov["def_pos"]))
         if p is not None:
-            found.add(p)
+            found.setdefault(p, None)
     return list(found)
 
 

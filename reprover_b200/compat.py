@@ -46,11 +46,16 @@ class _RefIndexedCorpus(_Bag):
     pass
 
 
+class _RefContext(_Bag):
+    pass
+
+
 _MAP = {
     ("common", "IndexedCorpus"): _RefIndexedCorpus,
     ("common", "Corpus"): _RefCorpus,
     ("common", "File"): _RefFile,
     ("common", "Premise"): _RefPremise,
+    ("common", "Context"): _RefContext,
 }
 
 
@@ -133,6 +138,31 @@ def load_reference_index(path_or_bytes) -> IndexedCorpus:
     with fh:
         ref = _Unpickler(fh).load()
     return IndexedCorpus(convert_corpus(ref.corpus), ref.embeddings)
+
+
+def load_reference_predictions(path_or_bytes) -> List[Dict[str, Any]]:
+    """Load a retrieval predictions pickle in the reference's layout (`dump_reference_predictions`, or the reference's
+    own `predictions.pickle`) with `context` as `reprover_b200.corpus.Context` and premises as `Premise`."""
+    from .corpus import Context
+
+    fh = io.BytesIO(path_or_bytes) if isinstance(path_or_bytes, (bytes, bytearray)) else open(path_or_bytes, "rb")
+    with fh:
+        ref = _Unpickler(fh).load()
+    conv: Dict[int, Premise] = {}
+
+    def premise(p: Any) -> Premise:
+        q = conv.get(id(p))
+        if q is None:
+            q = conv[id(p)] = _premise(p)
+        return q
+
+    out = []
+    for rec in ref:
+        c = rec["context"]
+        out.append({**rec, "context": Context(c.path, c.theorem_full_name, _pos(c.theorem_pos), c.state),
+                    "all_pos_premises": [premise(p) for p in rec["all_pos_premises"]],
+                    "retrieved_premises": [premise(p) for p in rec["retrieved_premises"]]})
+    return out
 
 
 # ------------------------------------------------------------------------------------------ export

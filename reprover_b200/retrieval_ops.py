@@ -205,6 +205,23 @@ def nearest_premises_device(corpus, premise_embeddings: Union[torch.Tensor, Inde
     if dev.type != "cuda":
         raise RuntimeError("get_nearest_premises needs the embeddings on a CUDA device")
     _check_k(k)
+    nq = batch_context_emb.shape[0]
+    stage = _result_staging(nq, k)
+    nearest_premises_enqueue(corpus, premise_embeddings, batch_context, batch_context_emb, k, stage)
+    # one synchronisation for the three results (pinned staging, asynchronous copies)
+    torch.cuda.current_stream(dev).synchronize()
+    return nearest_premises_collect(corpus, stage, nq, k)
+
+
+def nearest_premises_enqueue(corpus, premise_embeddings: Union[torch.Tensor, IndexHandle], batch_context,
+                             batch_context_emb: torch.Tensor, k: int, stage: Tuple[torch.Tensor, ...]) -> None:
+    """The device half of `nearest_premises_device`: access masks, the masked top-k, and asynchronous copies of
+    (counts, indices, fp32 scores) into the pinned host buffers `stage` (see `result_staging`).  Returns without
+    waiting; the results are valid once the current stream has reached this point."""
+    dev = batch_context_emb.device
+    if dev.type != "cuda":
+        raise RuntimeError("get_nearest_premises needs the embeddings on a CUDA device")
+    _check_k(k)
     q = batch_context_emb.to(torch.bfloat16)
     e = premise_embeddings
     if not isinstance(e, IndexHandle):
@@ -216,13 +233,15 @@ def nearest_premises_device(corpus, premise_embeddings: Union[torch.Tensor, Inde
     assert len(batch_context) == q.shape[0] and n_rows == len(corpus.all_premises)
     mask = _device_mask(corpus, batch_context, dev)
     scores, idx, counts = sim_topk(q, e, k, access_mask=mask)
-    # one synchronisation for the three results (pinned staging, asynchronous copies)
     nq = q.shape[0]
-    stage = _result_staging(nq, k)
     stage[0][:nq].copy_(counts, non_blocking=True)
     stage[1][:nq].copy_(idx, non_blocking=True)
     stage[2][:nq].copy_(scores, non_blocking=True)
-    torch.cuda.current_stream(dev).synchronize()
+
+
+def nearest_premises_collect(corpus, stage: Tuple[torch.Tensor, ...], nq: int, k: int):
+    """The host half: premises and Python-float scores from the staged results of `nq` queries.  Raises ValueError
+    when a query had fewer than k accessible premises (common.py:323-324)."""
     if bool((stage[0][:nq] < k).any()):
         raise ValueError
     idx_h = stage[1][:nq].tolist()
@@ -230,6 +249,12 @@ def nearest_premises_device(corpus, premise_embeddings: Union[torch.Tensor, Inde
     premises = corpus.all_premises
     results = [[premises[i] for i in row] for row in idx_h]
     return results, scores_h
+
+
+def result_staging(nq: int, k: int) -> Tuple[torch.Tensor, ...]:
+    """Fresh pinned host buffers (counts, indices, fp32 scores) for `nq` queries of `nearest_premises_enqueue`."""
+    return (torch.empty(nq, dtype=torch.int32, pin_memory=True), torch.empty(nq, k, dtype=torch.int64, pin_memory=True),
+            torch.empty(nq, k, dtype=torch.float32, pin_memory=True))
 
 
 _staging = {}

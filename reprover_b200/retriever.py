@@ -40,9 +40,11 @@ class B200PremiseRetriever:
     def __init__(self, model_name: str, lr: float = 0.0, warmup_steps: int = 0, max_seq_len: int = 2048,
                  num_retrieved: int = 100, device: Union[int, str, torch.device, None] = None,
                  dtype: Optional[torch.dtype] = None, max_tokens_per_call: int = 1 << 18,
-                 output_dtype: Optional[torch.dtype] = None) -> None:
+                 output_dtype: Optional[torch.dtype] = None, config: Optional[dict] = None,
+                 state_dict: Optional[dict] = None) -> None:
         """`model_name` is an HF checkpoint directory (config.json + model.safetensors) or a hub id that
-        is available in the local HF cache."""
+        is available in the local HF cache.  With `config` and `state_dict` (HF `T5EncoderModel` names) the
+        encoder is built from those instead, and `model_name` is only recorded."""
         if device is None:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else "cpu"
         device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
@@ -73,7 +75,7 @@ class B200PremiseRetriever:
         if self.dtype not in (torch.bfloat16, torch.float32):
             raise NotImplementedError(f"output dtype {self.dtype} is not supported (bf16 or fp32)")
         self.model_name = model_name
-        cfg, sd = load_hf_checkpoint(model_name)
+        cfg, sd = (config, state_dict) if state_dict is not None else load_hf_checkpoint(model_name)
         self.encoder = T5EncoderEngine(cfg, sd, device, max_tokens_per_call=max_tokens_per_call)
         self._index_handle = None      # rpx_index over the bf16 copy of corpus_embeddings
         self._index_source = None      # (tensor identity, version) the handle was built from
@@ -88,6 +90,20 @@ class B200PremiseRetriever:
     @classmethod
     def load_hf(cls, ckpt_path: str, max_seq_len: int, device, dtype=None) -> "B200PremiseRetriever":
         return cls(ckpt_path, 0.0, 0, max_seq_len, 100, device=device, dtype=dtype)
+
+    @classmethod
+    def load(cls, ckpt_path: str, device, freeze: bool = True, config: Optional[dict] = None) -> "B200PremiseRetriever":
+        """Reference `PremiseRetriever.load` (retrieval/model.py:49-50, common.py:load_checkpoint): a Lightning `.ckpt`
+        written by the reference's training, or a DeepSpeed ZeRO checkpoint directory.  `model_name`, `lr`,
+        `warmup_steps`, `max_seq_len` and `num_retrieved` come from the checkpoint's hyper-parameters; the encoder
+        config from `config`, else `model_name`'s cached config, else the weights' shapes
+        (`reprover_b200.checkpoint`).  `freeze` is accepted for parity: the engine keeps no gradients."""
+        from .checkpoint import load_retriever_checkpoint
+
+        cfg, sd, hp = load_retriever_checkpoint(ckpt_path, config)
+        return cls(hp.get("model_name") or ckpt_path, float(hp.get("lr", 0.0)), int(hp.get("warmup_steps", 0)),
+                   int(hp.get("max_seq_len", 2048)), int(hp.get("num_retrieved", 100)), device=device,
+                   config=cfg, state_dict=sd)
 
     @property
     def corpus_embeddings(self) -> Optional[torch.Tensor]:

@@ -143,3 +143,59 @@ def random_unit_rows(n: int, d: int, seed: int, device, dtype=None, chunk: int =
         x = torch.randn(hi - lo, d, generator=g, device=device, dtype=torch.float32)
         out[lo:hi] = torch.nn.functional.normalize(x, dim=1).to(dtype)
     return out
+
+
+def write_leandojo_dataset(root: str, n_files: int = 8, premises_per_file: int = 40, theorems: Tuple[int, int, int] = (6, 3, 3),
+                           tactics_per_theorem: Tuple[int, int] = (1, 4), state_len: Tuple[int, int] = (16, 400),
+                           premise_len: Tuple[int, int] = (16, 300), min_accessible: int = 0, seed: int = SEED) -> str:
+    """A seeded LeanDojo-layout dataset under `root`: `corpus.jsonl` and `random/{train,val,test}.json`; returns the
+    split directory (`data_path`; the corpus is `<data_path>/../corpus.jsonl`).
+
+    File i imports file i-1, so it sees every earlier file.  Premise j of a file spans lines 10j+1 .. 10j+5.
+    `theorems` is the number of theorems per split, each in a file whose imports hold at least `min_accessible`
+    premises, with `tactics_per_theorem` (inclusive range) traced tactics.  States and premise code are random
+    printable ASCII (`synth_byte_strings`, lengths in the given inclusive ranges); states start with the turnstile.
+    Every tactic's provenances name 0-3 premises its theorem can see, located at a position inside them, and about
+    one tactic in four also names a position no premise covers (the reference skips it when collecting positives)."""
+    rng = np.random.default_rng(seed)
+    pdata, poff = synth_premises(n_files * premises_per_file, seed=seed + 1, min_len=premise_len[0],
+                                 max_len=premise_len[1])
+    bodies = [s.decode() for s in split_strings(pdata, poff)]
+    os.makedirs(os.path.join(root, "random"), exist_ok=True)
+    with open(os.path.join(root, "corpus.jsonl"), "w") as fh:
+        for f in range(n_files):
+            premises = [{"full_name": f"Synth.F{f}.p{j}", "code": f"theorem p{j} : {bodies[f * premises_per_file + j]}",
+                         "start": [10 * j + 1, 1], "end": [10 * j + 5, 1], "kind": "theorem"}
+                        for j in range(premises_per_file)]
+            fh.write(json.dumps({"path": f"Synth/F{f}.lean", "imports": [f"Synth/F{f - 1}.lean"] if f else [],
+                                 "premises": premises}) + "\n")
+    first_file = min(n_files - 1, -(-min_accessible // premises_per_file))
+    n_tac = rng.integers(tactics_per_theorem[0], tactics_per_theorem[1] + 1, size=sum(theorems))
+    sdata, soff = synth_states(int(n_tac.sum()), seed=seed + 2, min_len=state_len[0], max_len=state_len[1])
+    states = iter(s.decode() for s in split_strings(sdata, soff))
+    t_all = 0
+    for split, count in zip(("train", "val", "test"), theorems):
+        thms = []
+        for t in range(count):
+            f = int(rng.integers(first_file, n_files))
+            line = 10 * int(rng.integers(0, premises_per_file + 1)) + 3
+            visible = f * premises_per_file + (line - 3) // 10     # imported files + own premises ending before line
+            tactics = []
+            for _ in range(int(n_tac[t_all])):
+                prov = []
+                for g in rng.choice(visible, size=min(visible, int(rng.integers(0, 4))), replace=False).tolist():
+                    gf, gj = divmod(int(g), premises_per_file)
+                    prov.append({"full_name": f"Synth.F{gf}.p{gj}", "def_path": f"Synth/F{gf}.lean",
+                                 "def_pos": [10 * gj + 2, 1], "def_end_pos": [10 * gj + 5, 1]})
+                if rng.random() < 0.25:
+                    prov.append({"full_name": "Synth.missing", "def_path": f"Synth/F{f}.lean",
+                                 "def_pos": [10 * premises_per_file + 50, 1], "def_end_pos": [10 * premises_per_file + 51, 1]})
+                tactics.append({"tactic": "simp", "annotated_tactic": ["simp [<a>x</a>]", prov],
+                                "state_before": next(states), "state_after": "no goals"})
+            t_all += 1
+            thms.append({"url": "https://example.org/synth", "commit": "0" * 40, "file_path": f"Synth/F{f}.lean",
+                         "full_name": f"Synth.{split}{t}", "start": [line, 1], "end": [line + 8, 1],
+                         "traced_tactics": tactics})
+        with open(os.path.join(root, "random", f"{split}.json"), "w") as fh:
+            json.dump(thms, fh)
+    return os.path.join(root, "random")
