@@ -167,6 +167,11 @@ int rpx_encoder_set_latency_tokens(rpx_encoder* enc, int32_t max_tokens);
  * CPU test-suite can pin the table the attention kernel uses against the HF code. */
 int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num_buckets, int32_t max_distance);
 
+/* The unidirectional bucket the decoder's self-attention uses (HF `_relative_position_bucket(bidirectional=False)`):
+ * relative_position = key - query <= 0 spreads over all `num_buckets`, positive positions fall in bucket 0.  Requires
+ * max_distance > num_buckets / 2.  Pure host function. */
+int32_t rpx_t5_relative_bucket_unidirectional(int32_t relative_position, int32_t num_buckets, int32_t max_distance);
+
 /* Debug / parity hook: when non-NULL, every encode call also writes the fp32
  * residual stream after the embedding and after each block to
  * d_hidden[(layer) * n_tokens * d_model ...] (num_layers + 1 slabs, packed tokens). */
@@ -179,6 +184,76 @@ int rpx_encoder_set_profiling(rpx_encoder* enc, int32_t enable);
 /* Synchronises the recorded events; adds elapsed ms / launch counts since the
  * last read into ms[RPX_N_KERNEL_CLASSES], launches[RPX_N_KERNEL_CLASSES]. */
 int rpx_encoder_read_profile(rpx_encoder* enc, float* h_ms, int64_t* h_launches);
+
+/* ------------------------------------------------------------------- tactic generator
+ * The teacher-forced forward of the reference's tactic generator, a `T5ForConditionalGeneration` (ByT5-small:
+ * 12 encoder and 4 decoder layers):
+ *     self.generator(input_ids=state_ids, attention_mask=state_mask, labels=tactic_ids)   generation/model.py:101-111
+ * giving `.loss` and `.logits`.  The encoder half runs on an rpx_encoder built from the same checkpoint's
+ * `encoder.*` keys; the decoder handle holds the decoder layers, the cross-attention K / V projections of all of
+ * them and the output head.  Weights are packed as the encoder's are (bf16, each RMSNorm weight folded into the B
+ * operand of the GEMM that follows it, FFN-up interleaved in 128-row blocks); in addition
+ *   - the cross K / V weights of all decoder layers form one [num_layers * 2 * heads * d_kv, d_model] matrix with
+ *     encoder.final_layer_norm folded in, applied once per call to the encoder's last residual stream;
+ *   - decoder.final_layer_norm (and, with scale_decoder_outputs, d_model ** -0.5) is folded into the head rows.
+ * HF key of each member on the right (i = decoder layer). */
+typedef struct {
+  const float* d_shared;         /* shared.weight (the decoder's embedding)                      [vocab, d_model] */
+  const float* d_rel_bias;       /* decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight [buckets, heads] */
+  const float* d_final_ln;       /* decoder.final_layer_norm.weight                              [d_model]        */
+  const float* d_enc_final_ln;   /* encoder.final_layer_norm.weight                              [d_model]        */
+  const float* d_head;           /* lm_head.weight, or shared.weight when the embeddings are tied [vocab, d_model] */
+  const float* const* h_q;       /* decoder.block.i.layer.0.SelfAttention.q.weight               [heads*d_kv, d_model] */
+  const float* const* h_k;       /* ...k.weight                                                                    */
+  const float* const* h_v;       /* ...v.weight                                                                    */
+  const float* const* h_o;       /* ...o.weight                                                  [d_model, heads*d_kv] */
+  const float* const* h_ln0;     /* decoder.block.i.layer.0.layer_norm.weight                    [d_model]        */
+  const float* const* h_cq;      /* decoder.block.i.layer.1.EncDecAttention.q.weight             [heads*d_kv, d_model] */
+  const float* const* h_ck;      /* ...k.weight                                                                    */
+  const float* const* h_cv;      /* ...v.weight                                                                    */
+  const float* const* h_co;      /* ...o.weight                                                  [d_model, heads*d_kv] */
+  const float* const* h_ln1;     /* decoder.block.i.layer.1.layer_norm.weight                    [d_model]        */
+  const float* const* h_wi0;     /* decoder.block.i.layer.2.DenseReluDense.wi_0.weight           [d_ff, d_model]  */
+  const float* const* h_wi1;     /* ...wi_1.weight                                                                 */
+  const float* const* h_wo;      /* ...wo.weight                                                 [d_model, d_ff]  */
+  const float* const* h_ln2;     /* decoder.block.i.layer.2.layer_norm.weight                    [d_model]        */
+} rpx_t5_decoder_weights;
+
+typedef struct rpx_t5_decoder rpx_t5_decoder; /* opaque */
+
+/* `cfg` describes the decoder: num_layers = the checkpoint's num_decoder_layers, everything else as the encoder's.
+ * 0 for a config rpx_t5_decoder_create rejects. */
+size_t rpx_t5_decoder_packed_bytes(const rpx_t5_config* cfg);
+/* Packs the weights into d_packed (synchronises `stream`; the fp32 weights may be freed on return).
+ *   scale_decoder_outputs  nonzero: logits are scaled by d_model ** -0.5 (HF T5 with tied embeddings)
+ *   start_token_id         decoder_start_token_id, which must equal the pad id (HF `_shift_right` feeds both) */
+int rpx_t5_decoder_create(const rpx_t5_config* cfg, const rpx_t5_decoder_weights* w, int32_t scale_decoder_outputs,
+                          int32_t start_token_id, void* d_packed, size_t packed_bytes, void* stream,
+                          rpx_t5_decoder** out);
+int rpx_t5_decoder_destroy(rpx_t5_decoder* dec);
+
+/* Workspace of one rpx_seq2seq_forward call on [batch, in_len] states and [batch, out_len] labels (0 when `dec`
+ * and `enc` do not fit together). */
+size_t rpx_seq2seq_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch, int32_t in_len,
+                                   int32_t out_len);
+/* HF `T5ForConditionalGeneration(input_ids, attention_mask, labels)` (teacher forcing), on the throughput tiles:
+ *   d_input_ids       int64 [batch, in_len] state ids; d_attention_mask int64 [batch, in_len] right-padded prefix mask
+ *                     with at least one token per row (RPX_ERR_MASK otherwise), or NULL: every position is a token
+ *   d_labels          int64 [batch, out_len]: target ids in [0, vocab) or -100 (ignored)
+ *   d_logits          optional fp32 [batch, out_len, vocab]
+ *   d_seq_logprob     fp64 [batch]: sum over the counted positions of log_softmax(logits)[label]
+ *   d_seq_count       int32 [batch]: the counted positions (labels != -100)
+ * Decoder inputs are HF `_shift_right(labels)`: start token, then labels[:, :-1] with -100 fed as the pad id.  Row
+ * b's decoder length is the last position whose label is not -100, plus one; positions at or past it are never
+ * computed (causality: no counted position sees them) and their logits are written as zeros, where HF computes
+ * values that its loss ignores.  HF's loss is -sum(seq_logprob) / sum(seq_count).  Every output row depends on its
+ * own row of the inputs alone.  Ids outside [0, vocab) in d_input_ids give RPX_ERR_INVALID (after the call ran
+ * with id 0 in their place); labels that are neither -100 nor in [0, vocab) give RPX_ERR_INVALID before anything
+ * runs.  Synchronises `stream` twice (lengths, then the id check). */
+int rpx_seq2seq_forward(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
+                        const int64_t* d_attention_mask, int32_t batch, int32_t in_len, const int64_t* d_labels,
+                        int32_t out_len, float* d_logits, double* d_seq_logprob, int32_t* d_seq_count,
+                        void* d_workspace, size_t workspace_bytes, void* stream);
 
 /* --------------------------------------------------------------- similarity + top-k
  * Replaces the matmul + argsort half of `Corpus.get_nearest_premises`
@@ -339,6 +414,22 @@ int rpx_debug_attention_lut(const float* d_rel_bias, int32_t n_heads, int32_t re
 int rpx_debug_attention(int32_t latency, const void* d_qkv, void* d_out, const int32_t* d_cu_seqlens,
                         const float* d_lut, int32_t n_tokens, int32_t n_seqs, int32_t max_len,
                         int32_t n_heads, int32_t rel_max_distance, void* stream);
+
+/* rpx_debug_attention_lut with the bucket direction chosen: bidirectional != 0 is the encoder's table, 0 the
+ * decoder's (unidirectional buckets; requires rel_max_distance > rel_buckets / 2). */
+int rpx_debug_attention_lut_ex(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets,
+                               int32_t rel_max_distance, int32_t bidirectional, float* d_lut, void* stream);
+enum { RPX_ATTN_BIDIRECTIONAL = 0, RPX_ATTN_CAUSAL = 1, RPX_ATTN_CROSS = 2 };
+/* The attention kernel in any of its modes, launched as the generator's forward launches it (throughput PDL
+ * scope for n_q_tokens).
+ *   RPX_ATTN_BIDIRECTIONAL, RPX_ATTN_CAUSAL  d_q = qkv [n_q_tokens, 3 * n_heads * 64] as rpx_debug_attention; d_kv and
+ *           d_cu_kv are ignored (NULL); causal: key j visible to query i iff j <= i
+ *   RPX_ATTN_CROSS  d_q [n_q_tokens, n_heads * 64] queries; d_kv [n_kv_tokens, 2 * n_heads * 64] k | v with its own
+ *           d_cu_kv [n_seqs + 1]; every query of sequence s sees all keys of sequence s; no bias, d_lut ignored
+ *   d_out   [n_q_tokens, n_heads * 64] bf16; max_len >= every query sequence's length.  Does not synchronise. */
+int rpx_debug_attention_ex(int32_t mode, const void* d_q, const void* d_kv, void* d_out, const int32_t* d_cu_q,
+                           const int32_t* d_cu_kv, const float* d_lut, int32_t n_q_tokens, int32_t n_kv_tokens,
+                           int32_t n_seqs, int32_t max_len, int32_t n_heads, int32_t rel_max_distance, void* stream);
 
 #ifdef __cplusplus
 }

@@ -72,6 +72,30 @@ class T5Weights(C.Structure):
     ]
 
 
+class T5DecoderWeights(C.Structure):
+    _fields_ = [
+        ("d_shared", C.c_void_p),
+        ("d_rel_bias", C.c_void_p),
+        ("d_final_ln", C.c_void_p),
+        ("d_enc_final_ln", C.c_void_p),
+        ("d_head", C.c_void_p),
+        ("h_q", _PP),
+        ("h_k", _PP),
+        ("h_v", _PP),
+        ("h_o", _PP),
+        ("h_ln0", _PP),
+        ("h_cq", _PP),
+        ("h_ck", _PP),
+        ("h_cv", _PP),
+        ("h_co", _PP),
+        ("h_ln1", _PP),
+        ("h_wi0", _PP),
+        ("h_wi1", _PP),
+        ("h_wo", _PP),
+        ("h_ln2", _PP),
+    ]
+
+
 # name -> (restype, argtypes); mirrors include/rpx.h one to one.
 _SIGNATURES = {
     "rpx_last_error": (C.c_char_p, []),
@@ -90,6 +114,15 @@ _SIGNATURES = {
                                         C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_encoder_set_latency_tokens": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_t5_relative_bucket": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
+    "rpx_t5_relative_bucket_unidirectional": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32]),
+    "rpx_t5_decoder_packed_bytes": (C.c_size_t, [C.POINTER(T5Config)]),
+    "rpx_t5_decoder_create": (C.c_int, [C.POINTER(T5Config), C.POINTER(T5DecoderWeights), C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "rpx_t5_decoder_destroy": (C.c_int, [C.c_void_p]),
+    "rpx_seq2seq_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
+    "rpx_seq2seq_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                      C.c_void_p]),
     "rpx_encoder_set_debug_hidden": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rpx_encoder_set_profiling": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_encoder_read_profile": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
@@ -129,12 +162,21 @@ _SIGNATURES = {
     "rpx_debug_attention_lut": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "rpx_debug_attention": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                       C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "rpx_debug_attention_lut_ex": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                             C.c_void_p]),
+    "rpx_debug_attention_ex": (C.c_int, [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_void_p]),
 }
 
 RPX_EGEMM_QKV = 0
 RPX_EGEMM_OPROJ = 1
 RPX_EGEMM_FFN_UP = 2
 RPX_EGEMM_FFN_DOWN = 3
+
+RPX_ATTN_BIDIRECTIONAL = 0
+RPX_ATTN_CAUSAL = 1
+RPX_ATTN_CROSS = 2
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -17,6 +17,17 @@
 //              (tensor maps over the packed qkv activation matrix, box 64 columns x 64 rows).
 // Small tiles keep many CTAs per state on the latency path and several CTAs per SM, which hide each
 // other's softmax behind their tensor-core work.
+//
+// Three modes (compile-time), one kernel body:
+//   kBidirectional  the encoder: keys 0 <= j < len of the query's own sequence, bias lut[h][clamp(j - i) + R]
+//                   (HF bidirectional buckets).  q, k, v are column blocks of one qkv matrix.
+//   kCausal         decoder self-attention (HF is_decoder): keys 0 <= j <= i, the decoder's own bias table built
+//                   from unidirectional buckets (same LUT convention; every delta <= -R falls in the last bucket, so
+//                   the clamp is exact).  Key tiles wholly above the diagonal are neither loaded nor computed.
+//   kCross          decoder cross-attention (EncDecAttention): queries from the decoder's packed tokens, keys and
+//                   values from the encoder's packed tokens with their own cu_seqlens; query row i of sequence b
+//                   sees all len_enc(b) keys, no bias, no causal mask.
+// In every mode key 0 lies in each query tile's first step, so the running maxima are finite from then on.
 #include "rpx_common.cuh"
 #include "rpx_kernels.cuh"
 #include "rpx_ptx.cuh"
@@ -47,10 +58,15 @@ RPX_DEVICE float fast_exp2(float x) {
   return y;
 }
 
+// Column offsets of head 0's q, k and v in the matrices tm_q / tm_kv map (head h adds 64 h); `cu_kv` is read
+// in kCross mode only (the self-attention modes take their keys from the query's own sequence).
+template <AttnMode MODE>
 __global__ void __launch_bounds__(kAttnThreads, 2)
 t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_kv,
                     __nv_bfloat16* __restrict__ out, const int32_t* __restrict__ cu_seqlens,
-                    const float* __restrict__ bias_lut, int n_heads, int R, int ld_out) {
+                    const int32_t* __restrict__ cu_kv, const float* __restrict__ bias_lut, int n_heads, int R,
+                    int ld_out, int q_col, int k_col, int v_col) {
+  constexpr bool kBias = MODE != AttnMode::kCross;
   const int seq = blockIdx.z, head = blockIdx.y, qt = blockIdx.x;
   // Under programmatic dependent launch this CTA may start while the QKV projection is still running.
   // cu_seqlens and bias_lut were complete before the first kernel of the chain started, so the whole
@@ -61,6 +77,8 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
   const int len = cu_seqlens[seq + 1] - t0;
   const int q0 = qt * kQT;
   if (q0 >= len) return;  // whole CTA
+  const int kv0 = MODE == AttnMode::kCross ? cu_kv[seq] : t0;
+  const int kv_len = MODE == AttnMode::kCross ? cu_kv[seq + 1] - kv0 : len;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -74,10 +92,11 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
   uint64_t* bar_free = bars + 5;  // [2]: K / V buffer consumed by the warpgroup
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int inner = n_heads * kHD;
-  const int n_kt = (len + kKT - 1) / kKT;
+  // causal: the key tiles up to the diagonal one (the last query of the tile, or of the sequence)
+  const int n_kt = MODE == AttnMode::kCausal ? (min(len, q0 + kQT) + kKT - 1) / kKT : (kv_len + kKT - 1) / kKT;
 
-  for (int i = threadIdx.x; i < lut_w; i += kAttnThreads) sBias[i] = bias_lut[head * lut_w + i];
+  if (kBias)
+    for (int i = threadIdx.x; i < lut_w; i += kAttnThreads) sBias[i] = bias_lut[head * lut_w + i];
   if (warp == 4) {
     if (elect_one()) {
       mbar_init(bar_q, 1);
@@ -95,17 +114,17 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
   if (warp == 4) {
     // ------------------------------------------------------------------ TMA producer (one thread)
     if (elect_one()) {
-      const int kcol = inner + head * kHD, vcol = 2 * inner + head * kHD;
+      const int kcol = k_col + head * kHD, vcol = v_col + head * kHD;
       pdl_wait();
       mbar_arrive_expect_tx(bar_q, kTileBytes);
-      tma_load_2d(smem + kOffQ, &tm_q, bar_q, head * kHD, t0 + q0);
+      tma_load_2d(smem + kOffQ, &tm_q, bar_q, q_col + head * kHD, t0 + q0);
       for (int kt = 0; kt < n_kt; ++kt) {
         const int b = kt & 1;
         if (kt >= 2) mbar_wait<0>(&bar_free[b], ((kt >> 1) - 1) & 1);
         mbar_arrive_expect_tx(&bar_k[b], kTileBytes);
-        tma_load_2d(smem + kOffK + b * kTileBytes, &tm_kv, &bar_k[b], kcol, t0 + kt * kKT);
+        tma_load_2d(smem + kOffK + b * kTileBytes, &tm_kv, &bar_k[b], kcol, kv0 + kt * kKT);
         mbar_arrive_expect_tx(&bar_v[b], kTileBytes);
-        tma_load_2d(smem + kOffV + b * kTileBytes, &tm_kv, &bar_v[b], vcol, t0 + kt * kKT);
+        tma_load_2d(smem + kOffV + b * kTileBytes, &tm_kv, &bar_v[b], vcol, kv0 + kt * kKT);
       }
     }
   } else {
@@ -143,11 +162,18 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int key = kb + 8 * j + cq + e;
-          const bool ok = key < len;
-          const float b0 = sBias[min(max(key - qpos0 + R, 0), 2 * R)];
-          const float b1 = sBias[min(max(key - qpos1 + R, 0), 2 * R)];
-          sc[4 * j + e] = ok ? sc[4 * j + e] + b0 : -INFINITY;
-          sc[4 * j + 2 + e] = ok ? sc[4 * j + 2 + e] + b1 : -INFINITY;
+          const bool ok = key < kv_len;
+          const bool ok0 = MODE == AttnMode::kCausal ? ok && key <= qpos0 : ok;
+          const bool ok1 = MODE == AttnMode::kCausal ? ok && key <= qpos1 : ok;
+          if constexpr (kBias) {
+            const float b0 = sBias[min(max(key - qpos0 + R, 0), 2 * R)];
+            const float b1 = sBias[min(max(key - qpos1 + R, 0), 2 * R)];
+            sc[4 * j + e] = ok0 ? sc[4 * j + e] + b0 : -INFINITY;
+            sc[4 * j + 2 + e] = ok1 ? sc[4 * j + 2 + e] + b1 : -INFINITY;
+          } else {
+            sc[4 * j + e] = ok0 ? sc[4 * j + e] : -INFINITY;
+            sc[4 * j + 2 + e] = ok1 ? sc[4 * j + 2 + e] : -INFINITY;
+          }
           mx0 = fmaxf(mx0, sc[4 * j + e]);
           mx1 = fmaxf(mx1, sc[4 * j + 2 + e]);
         }
@@ -156,7 +182,8 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
       mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
       mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
       mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
-      // key 0 of the sequence lies in the first step, so the running maxima are finite from then on
+      // key 0 of the sequence lies in the first step (visible in every mode), so the running maxima are finite
+      // from then on
       const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
       const float scale0 = fast_exp2((m0 - mn0) * kLog2e), scale1 = fast_exp2((m1 - mn1) * kLog2e);  // 0 on the first step
       m0 = mn0;
@@ -214,31 +241,48 @@ t5_attention_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_const
   }
 }
 
+template <AttnMode MODE>
+int launch_mode(const AttnArgs& a, cudaStream_t stream) {
+  RPX_REQUIRE(a.d_kv == kHD, RPX_ERR_UNSUPPORTED, "attention: d_kv=%d (only 64 is implemented)", a.d_kv);
+  RPX_REQUIRE(a.n_seqs > 0 && a.max_len > 0 && a.q_rows > 0 && a.kv_rows > 0, RPX_ERR_INVALID, "attention: empty batch");
+  RPX_REQUIRE(a.n_seqs <= 65535 && a.n_heads <= 65535, RPX_ERR_UNSUPPORTED, "attention: grid limits exceeded");
+  DeviceInfo dev;
+  RPX_TRY(get_device_info(&dev));
+  CUtensorMap tm_q, tm_kv;
+  RPX_TRY(make_tmap_bf16_2d(&tm_kv, a.kv, (uint64_t)a.kv_rows, (uint64_t)a.kv_ld, (uint64_t)a.kv_ld, kKT));
+  RPX_TRY(make_tmap_bf16_2d(&tm_q, a.q, (uint64_t)a.q_rows, (uint64_t)a.q_ld, (uint64_t)a.q_ld, kQT));
+  const int R = MODE == AttnMode::kCross ? 0 : a.max_distance;
+  const size_t smem = attention_smem_bytes(R);
+  RPX_REQUIRE(smem <= 100 * 1024, RPX_ERR_UNSUPPORTED, "attention: bias table too large (%zu B of shared memory)", smem);
+  auto kern = t5_attention_kernel<MODE>;
+  static thread_local int configured = -1;  // per mode
+  if (configured != dev.device) {
+    RPX_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    configured = dev.device;
+  }
+  const dim3 grid((a.max_len + kQT - 1) / kQT, a.n_heads, a.n_seqs);
+  RPX_CUDA_OK(launch_pdl(kern, grid, dim3(kAttnThreads), smem, stream, pdl_enabled(), tm_q, tm_kv, a.out, a.cu_q,
+                         a.cu_kv, a.bias_lut, a.n_heads, R, a.ld_out, a.q_col, a.k_col, a.v_col));
+  return RPX_OK;
+}
+
 }  // namespace
 
 int launch_t5_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, const int32_t* cu_seqlens,
                         const float* bias_lut, int n_tokens, int n_seqs, int max_len, int n_heads, int d_kv,
                         int max_distance, cudaStream_t stream) {
-  RPX_REQUIRE(d_kv == kHD, RPX_ERR_UNSUPPORTED, "attention: d_kv=%d (only 64 is implemented)", d_kv);
-  RPX_REQUIRE(n_seqs > 0 && max_len > 0 && n_tokens > 0, RPX_ERR_INVALID, "attention: empty batch");
-  RPX_REQUIRE(n_seqs <= 65535 && n_heads <= 65535, RPX_ERR_UNSUPPORTED, "attention: grid limits exceeded");
   const int inner = n_heads * d_kv;
-  DeviceInfo dev;
-  RPX_TRY(get_device_info(&dev));
-  CUtensorMap tm_q, tm_kv;
-  RPX_TRY(make_tmap_bf16_2d(&tm_kv, qkv, (uint64_t)n_tokens, (uint64_t)3 * inner, (uint64_t)3 * inner, kKT));
-  RPX_TRY(make_tmap_bf16_2d(&tm_q, qkv, (uint64_t)n_tokens, (uint64_t)3 * inner, (uint64_t)3 * inner, kQT));
-  const size_t smem = attention_smem_bytes(max_distance);
-  RPX_REQUIRE(smem <= 100 * 1024, RPX_ERR_UNSUPPORTED, "attention: bias table too large (%zu B of shared memory)", smem);
-  static thread_local int configured = -1;
-  if (configured != dev.device) {
-    RPX_CUDA_OK(cudaFuncSetAttribute(t5_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    configured = dev.device;
+  AttnArgs a{qkv, n_tokens, 3 * inner, 0, qkv, n_tokens, 3 * inner, inner, 2 * inner, out, inner, cu_seqlens,
+             cu_seqlens, bias_lut, n_seqs, max_len, n_heads, d_kv, max_distance};
+  return launch_mode<AttnMode::kBidirectional>(a, stream);
+}
+
+int launch_t5_attention_mode(AttnMode mode, const AttnArgs& a, cudaStream_t stream) {
+  switch (mode) {
+    case AttnMode::kBidirectional: return launch_mode<AttnMode::kBidirectional>(a, stream);
+    case AttnMode::kCausal: return launch_mode<AttnMode::kCausal>(a, stream);
+    default: return launch_mode<AttnMode::kCross>(a, stream);
   }
-  const dim3 grid((max_len + kQT - 1) / kQT, n_heads, n_seqs);
-  RPX_CUDA_OK(launch_pdl(t5_attention_kernel, grid, dim3(kAttnThreads), smem, stream, pdl_enabled(), tm_q, tm_kv, out,
-                         cu_seqlens, bias_lut, n_heads, max_distance, inner));
-  return RPX_OK;
 }
 
 }  // namespace rpx

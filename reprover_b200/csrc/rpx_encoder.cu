@@ -20,36 +20,28 @@
 #include <new>
 #include <vector>
 
+#include "rpx_encoder.cuh"
 #include "rpx_gemm_launch.cuh"
 #include "rpx_kernels.cuh"
 
-namespace rpx {
-
 namespace {
 
-struct LayerW {
-  const __nv_bfloat16* qkv;  // [3*inner, D]   (ln0 folded)
-  const __nv_bfloat16* o;    // [D, inner]
-  const __nv_bfloat16* wi;   // [2*d_ff, D]    (ln1 folded; wi_0 / wi_1 interleaved in 128-row blocks)
-  const __nv_bfloat16* wo;   // [D, d_ff]
-};
-
-struct ProfRec {
-  int cls;
-  cudaEvent_t a, b;
-};
-
-}  // namespace
-
-}  // namespace rpx
-
-// T5 relative-position bucket, bidirectional (HF modeling_t5.py:189-234), float32 math
-// like the reference implementation.  Host function, exported for the CPU parity test.
-// Precondition (check_rel_attention): max_distance > num_buckets / 4, else the log-spaced branch divides by 0.
-extern "C" int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num_buckets, int32_t max_distance) {
-  int nb = num_buckets / 2;
-  int ret = relative_position > 0 ? nb : 0;
-  int n = relative_position < 0 ? -relative_position : relative_position;
+// T5 relative-position bucket (HF modeling_t5.py:189-234), float32 math like the reference implementation.
+// Bidirectional: half the buckets per sign, positive deltas in the upper half.  Unidirectional (the decoder):
+// every bucket for delta <= 0, and delta > 0 in bucket 0.
+// Precondition: max_distance > max_exact (num_buckets / 4, or / 2 unidirectional), else the log-spaced branch
+// divides by 0.
+int32_t relative_bucket(int32_t relative_position, int32_t num_buckets, int32_t max_distance, bool bidirectional) {
+  int nb = num_buckets;
+  int ret = 0;
+  int n;
+  if (bidirectional) {
+    nb = num_buckets / 2;
+    ret = relative_position > 0 ? nb : 0;
+    n = relative_position < 0 ? -relative_position : relative_position;
+  } else {
+    n = relative_position < 0 ? -relative_position : 0;
+  }
   const int max_exact = nb / 2;
   if (n < max_exact) return ret + n;
   float v = logf((float)n / (float)max_exact) / (float)log((double)max_distance / (double)max_exact) *
@@ -59,26 +51,16 @@ extern "C" int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num
   return ret + large;
 }
 
-struct rpx_encoder {
-  rpx_t5_config cfg;
-  int inner = 0;
-  int n_parts = 0;      // RMSNorm partial sums per row on the throughput path: one per 128-wide n-tile
-  int n_parts_lat = 0;  // ... on the latency path: one per 32-column chunk
-  int latency_tokens = 0;  // calls with at most this many packed tokens take the latency path (0: never)
-  size_t layer_bytes = 0;  // packed weights of one layer (qkv | o | wi | wo, contiguous from LayerW::qkv)
-  const float* emb = nullptr;
-  const float* final_ln = nullptr;
-  const float* bias_lut = nullptr;
-  std::vector<rpx::LayerW> layers;
-  float* debug_hidden = nullptr;
-  bool profiling = false;
-  std::vector<rpx::ProfRec> prof_pending;
-  std::vector<cudaEvent_t> event_pool;
-  float prof_ms[RPX_N_KERNEL_CLASSES] = {0};
-  int64_t prof_launches[RPX_N_KERNEL_CLASSES] = {0};
-  std::vector<int32_t> h_cu_tokens;
-  std::vector<int32_t> h_lens;
-};
+}  // namespace
+
+// Host functions, exported for the CPU parity tests.  Preconditions: check_rel_attention.
+extern "C" int32_t rpx_t5_relative_bucket(int32_t relative_position, int32_t num_buckets, int32_t max_distance) {
+  return relative_bucket(relative_position, num_buckets, max_distance, true);
+}
+extern "C" int32_t rpx_t5_relative_bucket_unidirectional(int32_t relative_position, int32_t num_buckets,
+                                                         int32_t max_distance) {
+  return relative_bucket(relative_position, num_buckets, max_distance, false);
+}
 
 namespace rpx {
 
@@ -118,10 +100,14 @@ PackedLayout packed_layout(const rpx_t5_config& c) {
   return L;
 }
 
-// The bucket formula takes log(max_distance / max_exact) with max_exact = buckets / 4, so max_distance must
-// exceed it; 2048 bounds the bias table the attention kernel keeps in shared memory.
-int check_rel_attention(int rel_buckets, int rel_max_distance) {
-  RPX_REQUIRE(rel_buckets >= 4 && rel_buckets % 4 == 0 && rel_max_distance > rel_buckets / 4 && rel_max_distance <= 2048,
+}  // namespace
+
+// The bucket formula takes log(max_distance / max_exact) with max_exact = buckets / 4 (bidirectional) or buckets / 2
+// (unidirectional), so max_distance must exceed it; 2048 bounds the bias table the attention kernel keeps in shared
+// memory.
+int check_rel_attention(int rel_buckets, int rel_max_distance, bool bidirectional) {
+  const int max_exact = bidirectional ? rel_buckets / 4 : rel_buckets / 2;
+  RPX_REQUIRE(rel_buckets >= 4 && rel_buckets % 4 == 0 && rel_max_distance > max_exact && rel_max_distance <= 2048,
               RPX_ERR_UNSUPPORTED, "unsupported relative attention config (%d buckets, max distance %d)", rel_buckets,
               rel_max_distance);
   return RPX_OK;
@@ -133,8 +119,10 @@ int validate_cfg(const rpx_t5_config* c) {
   RPX_REQUIRE(c->d_model % 64 == 0 && c->d_model > 0, RPX_ERR_UNSUPPORTED, "d_model=%d must be a multiple of 64", c->d_model);
   RPX_REQUIRE(c->d_ff % 128 == 0 && c->d_ff > 0, RPX_ERR_UNSUPPORTED, "d_ff=%d must be a multiple of 128", c->d_ff);
   RPX_REQUIRE(c->num_heads > 0 && c->num_layers > 0 && c->vocab_size > 0, RPX_ERR_INVALID, "bad config");
-  return check_rel_attention(c->rel_buckets, c->rel_max_distance);
+  return check_rel_attention(c->rel_buckets, c->rel_max_distance, true);
 }
+
+namespace {
 
 __global__ void bias_lut_kernel(const float* __restrict__ rel_bias, const int32_t* __restrict__ buckets,
                                 float* __restrict__ lut, int n_heads, int width) {
@@ -144,14 +132,13 @@ __global__ void bias_lut_kernel(const float* __restrict__ rel_bias, const int32_
   lut[i] = rel_bias[buckets[j] * n_heads + h];
 }
 
-// Relative-position bias LUT: lut[h][delta + R] = rel_bias[bucket(delta)][h] for delta = key - query in [-R, R].
-// The bucket table is computed on the host and staged through `d_buckets` (2R + 1 int32).  Synchronises `st`:
-// the host table is pageable and dies on return.  The caller has checked the config (check_rel_attention).
-int build_bias_lut(const float* d_rel_bias, int n_heads, int rel_buckets, int R, int32_t* d_buckets, float* d_lut,
-                   cudaStream_t st) {
+}  // namespace
+
+int build_bias_lut(const float* d_rel_bias, int n_heads, int rel_buckets, int R, bool bidirectional, int32_t* d_buckets,
+                   float* d_lut, cudaStream_t st) {
   const int width = 2 * R + 1;
   std::vector<int32_t> buckets(width);
-  for (int j = 0; j < width; ++j) buckets[j] = rpx_t5_relative_bucket(j - R, rel_buckets, R);
+  for (int j = 0; j < width; ++j) buckets[j] = relative_bucket(j - R, rel_buckets, R, bidirectional);
   RPX_CUDA_OK(cudaMemcpyAsync(d_buckets, buckets.data(), (size_t)width * 4, cudaMemcpyHostToDevice, st));
   bias_lut_kernel<<<ceil_div(n_heads * width, 256), 256, 0, st>>>(d_rel_bias, d_buckets, d_lut, n_heads, width);
   RPX_CUDA_OK(cudaGetLastError());
@@ -159,21 +146,6 @@ int build_bias_lut(const float* d_rel_bias, int n_heads, int rel_buckets, int R,
   return RPX_OK;
 }
 
-struct Workspace {
-  int32_t* cu_tokens;
-  int64_t* cu_bytes;
-  int32_t* ids;
-  int32_t* lens;
-  int32_t* flag;
-  float* h32;
-  __nv_bfloat16* h16;
-  __nv_bfloat16* qkv;
-  __nv_bfloat16* attn;
-  __nv_bfloat16* ffn;
-  float* ssA;
-  float* ssB;
-  size_t total;
-};
 
 Workspace carve(const rpx_encoder* e, uint8_t* base, int64_t T, int64_t S) {
   Workspace w{};
@@ -200,6 +172,8 @@ Workspace carve(const rpx_encoder* e, uint8_t* base, int64_t T, int64_t S) {
   w.total = off;
   return w;
 }
+
+namespace {
 
 struct Prof {
   rpx_encoder* e;
@@ -249,18 +223,8 @@ constexpr int kLatStages = 6;
 constexpr int kLatSmallM = 64;
 constexpr int kLatSmallStages = 12;
 constexpr int kLatSmallMMaxTokens = 384;
-// Calls of at most this many tokens run their kernel chain under programmatic dependent launch: it hides
-// the prologue of each kernel behind the tail of its predecessor, which matters while the tails are a
-// noticeable share of a kernel's time.
-constexpr int kPdlMaxTokens = 16384;
+}  // namespace
 
-struct PdlScope {
-  explicit PdlScope(bool on) { set_pdl_scope(on); }
-  ~PdlScope() { set_pdl_scope(false); }
-};
-
-// RMSNorm partial sums per row: one per 128 columns on the throughput path (EpiWsResidual: two per 256-wide
-// tile), one per 32-column chunk on the latency path.
 int ss_parts(int d_model, bool latency) { return ceil_div(d_model, latency ? 32 : 128); }
 
 // The encoder's four GEMMs, each on the tiles the forward pass uses for T tokens on the throughput or the
@@ -344,6 +308,8 @@ int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K,
   return launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(A, K, B, K, T, N, K, ep, st);
 }
 
+namespace {
+
 // One encoder block on the throughput or the latency path, each kernel under its profiling class.
 // `next_weights` (latency path, not the last layer; else null): the QKV projection occupies 18 x ceil(T/64) (or
 // 18 x ceil(T/128)) SMs for 6 heads, and the rest of the GPU fetches these `next_bytes` into L2.
@@ -377,19 +343,15 @@ int forward_layer(rpx_encoder* e, bool latency, const Workspace& ws, const Layer
   return RPX_OK;
 }
 
-// What forward() writes after the last block.
-//   kPooled  final RMSNorm + masked mean + L2 normalise: [S, D]
-//   kHidden  final RMSNorm of every token (`last_hidden_state`): [S, seq_len, D], rows past a sequence's length zeroed
-enum class OutKind { kPooled, kHidden };
+}  // namespace
 
-// The forward pass proper.  ws.ids / ws.cu_tokens are already populated on `st`.  `seq_len` is the padded row
-// length of a kHidden output (unused for kPooled).
 int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutKind kind, int seq_len, void* d_out,
             int out_dtype, cudaStream_t st) {
   const rpx_t5_config& c = e->cfg;
   const int D = c.d_model, inner = e->inner, F = c.d_ff;
-  // the latency path needs d_ff in 128-unit blocks for its split-B tiles (validate_cfg) and narrow-tile n
-  const bool latency = T <= e->latency_tokens && D % 32 == 0 && (3 * inner) % 32 == 0;
+  // the latency path needs d_ff in 128-unit blocks for its split-B tiles (validate_cfg) and narrow-tile n;
+  // kResidual hands its residual stream to GEMMs of the throughput path, so it never takes it
+  const bool latency = kind != OutKind::kResidual && T <= e->latency_tokens && D % 32 == 0 && (3 * inner) % 32 == 0;
   const int P = latency ? e->n_parts_lat : e->n_parts;
   PdlScope pdl_scope(latency || T <= kPdlMaxTokens);
   {
@@ -409,6 +371,7 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutK
                           prefetch ? e->layer_bytes : 0, T, S, max_len, st));
     RPX_TRY(dump(l + 1));
   }
+  if (kind == OutKind::kResidual) return RPX_OK;
   if (kind == OutKind::kHidden) {
     Prof p(e, st, 6);
     // the latency path pools with pool_partial_kernel: its order of the ss parts keeps the rows consistent with it
@@ -425,7 +388,6 @@ int forward(rpx_encoder* e, const Workspace& ws, int T, int S, int max_len, OutK
   return RPX_OK;
 }
 
-}  // namespace
 }  // namespace rpx
 
 using namespace rpx;
@@ -479,7 +441,7 @@ int rpx_encoder_create(const rpx_t5_config* cfg, const rpx_t5_weights* w, void* 
   e->emb = reinterpret_cast<const float*>(base + L.emb);
   e->final_ln = reinterpret_cast<const float*>(base + L.final_ln);
 
-  TRY_E(build_bias_lut(w->d_rel_bias, cfg->num_heads, cfg->rel_buckets, cfg->rel_max_distance,
+  TRY_E(build_bias_lut(w->d_rel_bias, cfg->num_heads, cfg->rel_buckets, cfg->rel_max_distance, true,
                        reinterpret_cast<int32_t*>(base + L.bucket_tmp), reinterpret_cast<float*>(base + L.bias_lut), st));
   e->bias_lut = reinterpret_cast<const float*>(base + L.bias_lut);
 
@@ -684,17 +646,23 @@ int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const
   }
 }
 
-int rpx_debug_attention_lut(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets, int32_t rel_max_distance,
-                            float* d_lut, void* stream) {
+int rpx_debug_attention_lut_ex(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets, int32_t rel_max_distance,
+                               int32_t bidirectional, float* d_lut, void* stream) {
   RPX_REQUIRE(d_rel_bias && d_lut, RPX_ERR_INVALID, "rpx_debug_attention_lut: null argument");
   RPX_REQUIRE(n_heads > 0, RPX_ERR_INVALID, "rpx_debug_attention_lut: n_heads=%d", n_heads);
-  RPX_TRY(check_rel_attention(rel_buckets, rel_max_distance));
+  RPX_TRY(check_rel_attention(rel_buckets, rel_max_distance, bidirectional != 0));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int32_t* d_buckets = nullptr;
   RPX_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&d_buckets), (size_t)(2 * rel_max_distance + 1) * 4, st));
-  const int rc = build_bias_lut(d_rel_bias, n_heads, rel_buckets, rel_max_distance, d_buckets, d_lut, st);
+  const int rc =
+      build_bias_lut(d_rel_bias, n_heads, rel_buckets, rel_max_distance, bidirectional != 0, d_buckets, d_lut, st);
   RPX_CUDA_OK(cudaFreeAsync(d_buckets, st));
   return rc;
+}
+
+int rpx_debug_attention_lut(const float* d_rel_bias, int32_t n_heads, int32_t rel_buckets, int32_t rel_max_distance,
+                            float* d_lut, void* stream) {
+  return rpx_debug_attention_lut_ex(d_rel_bias, n_heads, rel_buckets, rel_max_distance, 1, d_lut, stream);
 }
 
 int rpx_debug_attention(int32_t latency, const void* d_qkv, void* d_out, const int32_t* d_cu_seqlens,

@@ -343,6 +343,35 @@ struct EpiWsStoreF32 {
   }
 };
 
+// C[m, n] = acc * rs[m] (fp32).  The generator's output head (rpx_decoder.cu): the decoder's final RMSNorm weight is
+// folded into B, its row scale applied here.
+struct EpiWsStoreF32Scaled {
+  struct Params {
+    float* C;
+    int ldc;
+    RowScale rs;
+  };
+  static constexpr int kResBufs = 0;
+  Params p;
+  float rs0 = 0.f, rs1 = 0.f;
+  __device__ EpiWsStoreF32Scaled(const Params& p_, const ResStream&) : p(p_) {}
+  __device__ void prefetch(const FragCtx& c) {
+    rs0 = c.r0 < c.M ? p.rs.get(c.r0) : 0.f;
+    rs1 = c.r0 + 8 < c.M ? p.rs.get(c.r0 + 8) : 0.f;
+  }
+  __device__ void tile(const FragCtx& c, const float (&acc)[128]) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if (8 * j < c.n_cols) {
+        float* dst = p.C + (size_t)c.r0 * p.ldc + c.n0 + 8 * j + 2 * c.q;
+        if (c.r0 < c.M) *reinterpret_cast<float2*>(dst) = make_float2(acc[4 * j] * rs0, acc[4 * j + 1] * rs0);
+        if (c.r0 + 8 < c.M)
+          *reinterpret_cast<float2*>(dst + 8 * (size_t)p.ldc) = make_float2(acc[4 * j + 2] * rs1, acc[4 * j + 3] * rs1);
+      }
+    }
+  }
+};
+
 // C[m, n] = bf16(acc * rs[m]).  The QKV projection (RMSNorm folded: the weight into B, the row scale here).
 struct EpiWsStoreBF16 {
   using Params = EpiStoreBF16::Params;

@@ -14,6 +14,26 @@ int launch_t5_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, const int3
                         const float* bias_lut, int n_tokens, int n_seqs, int max_len, int n_heads, int d_kv,
                         int max_distance, cudaStream_t stream);
 
+// The kernel's three modes (rpx_attention.cu): the encoder's, decoder causal self-attention, cross-attention.
+enum class AttnMode : int { kBidirectional = 0, kCausal = 1, kCross = 2 };
+// One attention launch in any mode.  q: [q_rows, q_ld] bf16, head h's queries in columns [q_col + 64 h, +64);
+// kv: [kv_rows, kv_ld] bf16, keys / values of head h at k_col + 64 h / v_col + 64 h; out [*, ld_out] bf16, head h in
+// columns [64 h, 64 h + 64).  cu_q: the queries' sequences; cu_kv: the keys' (kCross only; the self modes use
+// cu_q).  bias_lut: [heads][2 max_distance + 1] (unused in kCross).  max_len: longest query sequence.
+struct AttnArgs {
+  const __nv_bfloat16* q;
+  int q_rows, q_ld, q_col;
+  const __nv_bfloat16* kv;
+  int kv_rows, kv_ld, k_col, v_col;
+  __nv_bfloat16* out;
+  int ld_out;
+  const int32_t* cu_q;
+  const int32_t* cu_kv;
+  const float* bias_lut;
+  int n_seqs, max_len, n_heads, d_kv, max_distance;
+};
+int launch_t5_attention_mode(AttnMode mode, const AttnArgs& args, cudaStream_t stream);
+
 // ---- rpx_elementwise.cu
 // ByT5 tokenisation of packed byte strings into packed token ids (byte + 3, EOS = 1 last,
 // truncated to max_seq_len including EOS).  cu_bytes / cu_tokens are [n_seqs + 1] device arrays.

@@ -118,16 +118,56 @@ def random_t5_state_dict(cfg: Dict, seed: int = SEED) -> Dict[str, "torch.Tensor
     return sd
 
 
+def random_t5_seq2seq_state_dict(cfg: Dict, seed: int = SEED) -> Dict[str, "torch.Tensor"]:
+    """fp32 encoder-decoder weights under HF `T5ForConditionalGeneration` key names: `random_t5_state_dict`'s
+    encoder plus the decoder (`num_decoder_layers`, default `num_layers`) and, unless the config ties the embeddings,
+    `lm_head.weight`.  Drawn from a second generator, so the encoder keys equal `random_t5_state_dict(cfg, seed)`.
+    The decoder's relative-attention bias is drawn apart from the encoder's, and the head apart from `shared`."""
+    import torch
+
+    sd = random_t5_state_dict(cfg, seed)
+    g = torch.Generator().manual_seed(seed + 7919)
+    D, F = cfg["d_model"], cfg["d_ff"]
+    H, dk = cfg["num_heads"], cfg["d_kv"]
+    inner = H * dk
+
+    def normal(shape, std):
+        return torch.randn(shape, generator=g, dtype=torch.float32) * std
+
+    sd["decoder.embed_tokens.weight"] = sd["shared.weight"]
+    sd["decoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"] = normal(
+        (cfg["relative_attention_num_buckets"], H), 0.5)
+    for i in range(int(cfg.get("num_decoder_layers") or cfg["num_layers"])):
+        for j, att in ((0, "SelfAttention"), (1, "EncDecAttention")):
+            a = f"decoder.block.{i}.layer.{j}."
+            sd[a + att + ".q.weight"] = normal((inner, D), (D * dk) ** -0.5)
+            sd[a + att + ".k.weight"] = normal((inner, D), D ** -0.5)
+            sd[a + att + ".v.weight"] = normal((inner, D), D ** -0.5)
+            sd[a + att + ".o.weight"] = normal((D, inner), inner ** -0.5)
+            sd[a + "layer_norm.weight"] = 1.0 + normal((D,), 0.1)
+        f = f"decoder.block.{i}.layer.2."
+        sd[f + "DenseReluDense.wi_0.weight"] = normal((F, D), D ** -0.5)
+        sd[f + "DenseReluDense.wi_1.weight"] = normal((F, D), D ** -0.5)
+        sd[f + "DenseReluDense.wo.weight"] = normal((D, F), F ** -0.5)
+        sd[f + "layer_norm.weight"] = 1.0 + normal((D,), 0.1)
+    sd["decoder.final_layer_norm.weight"] = 1.0 + normal((D,), 0.1)
+    if cfg.get("tie_word_embeddings", True) is False:
+        sd["lm_head.weight"] = normal((cfg["vocab_size"], D), D ** -0.5)
+    return sd
+
+
 def save_hf_checkpoint(path: str, cfg: Dict, state_dict: Dict) -> None:
     """Writes `config.json` + `model.safetensors` the way `save_pretrained` lays them out."""
     from safetensors.torch import save_file
 
     os.makedirs(path, exist_ok=True)
     hf_cfg = dict(cfg)
-    hf_cfg.update(architectures=["T5EncoderModel"], model_type="t5", is_encoder_decoder=True)
+    arch = "T5ForConditionalGeneration" if "decoder.final_layer_norm.weight" in state_dict else "T5EncoderModel"
+    hf_cfg.update(architectures=[arch], model_type="t5", is_encoder_decoder=True)
     with open(os.path.join(path, "config.json"), "w") as fh:
         json.dump(hf_cfg, fh, indent=1)
-    tensors = {k: v.contiguous() for k, v in state_dict.items() if k != "encoder.embed_tokens.weight"}
+    tensors = {k: v.contiguous() for k, v in state_dict.items()
+               if k not in ("encoder.embed_tokens.weight", "decoder.embed_tokens.weight")}
     save_file(tensors, os.path.join(path, "model.safetensors"), metadata={"format": "pt"})
 
 
