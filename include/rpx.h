@@ -255,6 +255,42 @@ int rpx_seq2seq_forward(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_
                         int32_t out_len, float* d_logits, double* d_seq_logprob, int32_t* d_seq_count,
                         void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* Workspace of one rpx_seq2seq_generate call (0 when the arguments are out of range or `dec` and `enc` do not fit
+ * together).  Dominated by the KV cache: num_layers * max_length * batch * num_beams * 3 * inner bf16. */
+size_t rpx_seq2seq_generate_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch,
+                                            int32_t in_len, int32_t num_beams, int32_t max_length);
+/* Optional record of every step of a generate call, for tests: step t (t < max_steps) writes
+ *   d_scores   [max_steps][R][vocab] fp32  the step's log-probs (num_beams == 1: the logits), R = batch * num_beams
+ *   d_parents  [max_steps][R] int32        the row each next-step row continues (global row)
+ *   d_tokens   [max_steps][R] int32        the token each next-step row appends
+ * Rows of a state whose search has ended are not written. */
+typedef struct rpx_generate_trace {
+  float* d_scores;
+  int32_t* d_parents;
+  int32_t* d_tokens;
+  int32_t max_steps;
+} rpx_generate_trace;
+/* HF `T5ForConditionalGeneration.generate(input_ids, attention_mask, num_beams, num_return_sequences, max_length,
+ * length_penalty, do_sample=False, early_stopping=False)` with one EOS id and no logits processor: HF 5.5's
+ * `_beam_search` (num_beams > 1) or greedy `_sample` (num_beams == 1), each state's beams decoded together over a KV
+ * cache, every search step on the device.
+ *   d_input_ids / d_attention_mask  as rpx_seq2seq_forward (the mask may be NULL: every position is a token)
+ *   d_sequences  int64 [batch * num_return, max_length]: row b * num_return + j is state b's j-th best hypothesis,
+ *                the decoder start id, its tokens, then the fill id (beam: pad id, or eos_id when the pad id is 0, as
+ *                HF's `output_fill_value`; greedy: the pad id).  Columns [0, *h_out_len) are HF's `sequences`.
+ *   d_scores     fp32 [batch * num_return]: HF's `sequences_scores` (beam search only; may be NULL for greedy)
+ *   h_out_len    host: 1 + the longest returned hypothesis;  h_steps (host, optional): the decoder steps HF runs
+ *                for this call (the step at which the last search ended).  The engine checks for completion every 8
+ *                steps, so it may run up to 15 more steps whose GEMMs do full work and change no result.
+ * Candidates are ranked by score, ties by flat index (beam * vocab + token) ascending.  Checks: 1 <= num_return <=
+ * num_beams <= 128, 2 num_beams <= vocab_size (beam search), max_length >= 2, eos_id in the vocabulary; a bad mask
+ * gives RPX_ERR_MASK, ids outside the vocabulary RPX_ERR_INVALID.  Synchronises `stream`. */
+int rpx_seq2seq_generate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
+                         const int64_t* d_attention_mask, int32_t batch, int32_t in_len, int32_t num_beams,
+                         int32_t num_return, int32_t max_length, double length_penalty, int32_t eos_id,
+                         int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                         const rpx_generate_trace* trace, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* --------------------------------------------------------------- similarity + top-k
  * Replaces the matmul + argsort half of `Corpus.get_nearest_premises`
  * (common.py:307-308) and the first-k walk at :316-322:
@@ -430,6 +466,16 @@ enum { RPX_ATTN_BIDIRECTIONAL = 0, RPX_ATTN_CAUSAL = 1, RPX_ATTN_CROSS = 2 };
 int rpx_debug_attention_ex(int32_t mode, const void* d_q, const void* d_kv, void* d_out, const int32_t* d_cu_q,
                            const int32_t* d_cu_kv, const float* d_lut, int32_t n_q_tokens, int32_t n_kv_tokens,
                            int32_t n_seqs, int32_t max_len, int32_t n_heads, int32_t rel_max_distance, void* stream);
+
+/* The generator's decode self-attention at step t, as rpx_seq2seq_generate launches it:
+ *   d_cache  [max_length][rows][3 * n_heads * 64] bf16 (q | k | v); query of row r: cache row t * rows + r
+ *   d_lin    [rows][max_length] int32: key / value p of row r (p = 0..t) is cache row p * rows + lin[r][p]; NULL: r
+ *   d_lut    the decoder's table (rpx_debug_attention_lut_ex, bidirectional = 0)
+ *   d_out    [rows, n_heads * 64] bf16 = softmax_p(q.k_p + lut[h][max(p - t, -R) + R]) v_p per head, unscaled.
+ * Does not synchronise. */
+int rpx_debug_decode_attention(const void* d_cache, const int32_t* d_lin, const float* d_lut, void* d_out, int32_t t,
+                               int32_t rows, int32_t max_length, int32_t n_heads, int32_t rel_max_distance,
+                               void* stream);
 
 #ifdef __cplusplus
 }

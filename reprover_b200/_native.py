@@ -96,6 +96,15 @@ class T5DecoderWeights(C.Structure):
     ]
 
 
+class GenerateTrace(C.Structure):
+    _fields_ = [
+        ("d_scores", C.c_void_p),
+        ("d_parents", C.c_void_p),
+        ("d_tokens", C.c_void_p),
+        ("max_steps", C.c_int32),
+    ]
+
+
 # name -> (restype, argtypes); mirrors include/rpx.h one to one.
 _SIGNATURES = {
     "rpx_last_error": (C.c_char_p, []),
@@ -123,6 +132,14 @@ _SIGNATURES = {
     "rpx_seq2seq_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                       C.c_void_p]),
+    "rpx_seq2seq_generate_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                                          C.c_int32]),
+    "rpx_seq2seq_generate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_size_t,
+                                       C.c_void_p]),
+    "rpx_debug_decode_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                             C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "rpx_encoder_set_debug_hidden": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rpx_encoder_set_profiling": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_encoder_read_profile": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64)]),

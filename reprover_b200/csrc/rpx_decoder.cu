@@ -52,6 +52,10 @@ struct rpx_t5_decoder {
   std::vector<rpx::DecLayerW> layers;
   std::vector<int32_t> h_lens;  // enc lens [B], enc flag, dec lens [B], dec flag
   std::vector<int32_t> h_cu;
+  // generate: pinned words the host polls (done-state counts of two step blocks, out_len, ids flag) and the events
+  // that mark them written
+  int32_t* h_poll = nullptr;
+  cudaEvent_t poll_ev[2] = {nullptr, nullptr};
 };
 
 namespace rpx {
@@ -287,6 +291,98 @@ int decoder_layer(const rpx_t5_decoder* d, const DecLayerW& w, int layer, const 
   return RPX_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- generate
+// Device buffers of one generate call over B states, nb beams, R = B nb rows.  Nothing here grows with the step:
+// the KV cache holds every step's q | k | v rows in place, [num_layers][max_length][R][3 inner] bf16.
+struct GenWs {
+  size_t enc_off, dec_off;
+  __nv_bfloat16* cross_kv;  // [B * in_len, n_kv]
+  __nv_bfloat16* cache;
+  float* logits;            // [R, vocab]
+  int32_t* tokens;          // [max_length][R]
+  int32_t* lin;             // [2][R][max_length]
+  float* run_score;         // [R]
+  float* fin_score;         // [2][R]
+  int32_t* fin_len;         // [2][R]
+  int32_t* fin_flag;        // [2][R]
+  int32_t* fin_seq;         // [2][R][max_length]
+  int32_t* state;           // [B][4]
+  int32_t* counters;        // done count, out_len, last step
+  size_t cache_layer;       // elements of one layer's cache
+  size_t total;
+};
+
+GenWs carve_gen(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, int64_t B, int64_t in_len, int64_t nb,
+                int64_t ML) {
+  GenWs w{};
+  const int64_t Te = B * in_len, R = B * nb;
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    uint8_t* p = base ? base + off : nullptr;
+    off = align_up(off + bytes, 256);
+    return p;
+  };
+  w.enc_off = off;
+  take(carve(e, nullptr, Te, B).total);
+  w.dec_off = off;
+  take(carve(e, nullptr, R, B).total);
+  w.cross_kv = (__nv_bfloat16*)take((size_t)Te * d->n_kv * 2);
+  w.cache_layer = (size_t)ML * R * 3 * d->inner;
+  w.cache = (__nv_bfloat16*)take(w.cache_layer * d->cfg.num_layers * 2);
+  w.logits = (float*)take((size_t)R * d->cfg.vocab_size * 4);
+  w.tokens = (int32_t*)take((size_t)ML * R * 4);
+  w.lin = (int32_t*)take(2 * (size_t)R * ML * 4);
+  w.run_score = (float*)take((size_t)R * 4);
+  w.fin_score = (float*)take(2 * (size_t)R * 4);
+  w.fin_len = (int32_t*)take(2 * (size_t)R * 4);
+  w.fin_flag = (int32_t*)take(2 * (size_t)R * 4);
+  w.fin_seq = (int32_t*)take(2 * (size_t)R * ML * 4);
+  w.state = (int32_t*)take((size_t)B * 16);
+  w.counters = (int32_t*)take(16);
+  w.total = off;
+  return w;
+}
+
+// One decoder step for all R rows at position t: embed the rows' current tokens, every layer on the latency-path
+// launchers (self-attention over the cache, cross-attention over the state's encoder tokens), then the head into
+// fp32 logits [R, vocab].
+int decode_step(const rpx_t5_decoder* d, const rpx_encoder* e, const GenWs& g, const Workspace& dw, const int32_t* cu_enc,
+                int T_enc, int B, int nb, int ML, int t, cudaStream_t st) {
+  const rpx_t5_config& c = d->cfg;
+  const int R = B * nb, D = c.d_model, inner = d->inner, F = c.d_ff, P = e->n_parts_lat;
+  const float inv_d = 1.0f / (float)D;
+  RPX_TRY(launch_embed(g.tokens + (size_t)t * R, d->emb, dw.h32, dw.h16, dw.ssA, R, P, R, D, st));
+  float* sa = dw.ssA;
+  float* sb = dw.ssB;
+  for (int l = 0; l < c.num_layers; ++l) {
+    const DecLayerW& w = d->layers[l];
+    __nv_bfloat16* cache = g.cache + g.cache_layer * l;
+    RPX_TRY(qkv_gemm(true, R, dw.h16, w.qkv, 3 * inner, D, RowScale{sa, P, R, inv_d, c.ln_eps},
+                     cache + (size_t)t * R * 3 * inner, nullptr, 0, st));
+    DecodeAttnArgs da{cache, nb > 1 ? g.lin + (size_t)(t & 1) * R * ML : nullptr, d->bias_lut, dw.attn, g.state, t, R,
+                      3 * inner, inner, c.num_heads, ML, c.rel_max_distance, nb};
+    RPX_TRY(launch_decode_attention(da, st));
+    RPX_TRY(oproj_gemm(true, R, dw.attn, w.o, D, inner, dw.h32, dw.h16, sb, st));
+    RPX_TRY(qkv_gemm(true, R, dw.h16, w.cq, inner, D, RowScale{sb, P, R, inv_d, c.ln_eps}, dw.qkv, nullptr, 0, st));
+    AttnArgs cross{dw.qkv, R, inner, 0, g.cross_kv, T_enc, d->n_kv, 2 * l * inner, (2 * l + 1) * inner, dw.attn, inner,
+                   dw.cu_tokens, cu_enc, nullptr, B, nb, c.num_heads, c.d_kv, 0};
+    RPX_TRY(launch_t5_attention_mode(AttnMode::kCross, cross, st));
+    RPX_TRY(oproj_gemm(true, R, dw.attn, w.co, D, inner, dw.h32, dw.h16, sa, st));
+    RPX_TRY(ffn_up_gemm(true, R, dw.h16, w.wi, 2 * F, D, RowScale{sa, P, R, inv_d, c.ln_eps}, dw.ffn, st));
+    RPX_TRY(ffn_down_gemm(true, R, dw.ffn, w.wo, D, F, dw.h32, dw.h16, sb, st));
+    float* tmp = sa;
+    sa = sb;
+    sb = tmp;
+  }
+  EpiWsStoreF32Scaled::Params ep{g.logits, c.vocab_size, RowScale{sa, P, R, inv_d, c.ln_eps}};
+  return launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(dw.h16, D, d->head, D, R, c.vocab_size, D, ep, st);
+}
+
+// Steps enqueued between two reads of the done-state count.
+constexpr int kPollSteps = 8;
+constexpr int kMaxBeams = 128;
+constexpr size_t kMaxStepSmem = 227 * 1024 - 16 * 1024;  // the beam step's candidate keys, beside its static arrays
+
 }  // namespace
 }  // namespace rpx
 
@@ -388,6 +484,10 @@ int rpx_t5_decoder_create(const rpx_t5_config* cfg, const rpx_t5_decoder_weights
 }
 
 int rpx_t5_decoder_destroy(rpx_t5_decoder* dec) {
+  if (!dec) return RPX_OK;
+  if (dec->h_poll) cudaFreeHost(dec->h_poll);
+  for (cudaEvent_t ev : dec->poll_ev)
+    if (ev) cudaEventDestroy(ev);
   delete dec;
   return RPX_OK;
 }
@@ -499,6 +599,150 @@ int rpx_seq2seq_forward(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_
   RPX_CUDA_OK(cudaStreamSynchronize(st));
   RPX_REQUIRE((flag & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", V);
   return RPX_OK;
+}
+
+size_t rpx_seq2seq_generate_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch,
+                                            int32_t in_len, int32_t num_beams, int32_t max_length) {
+  if (!dec || !enc || batch <= 0 || in_len <= 0 || num_beams <= 0 || num_beams > kMaxBeams || max_length < 2 ||
+      check_pair(dec, enc) != RPX_OK)
+    return 0;
+  return carve_gen(dec, enc, nullptr, batch, in_len, num_beams, max_length).total;
+}
+
+int rpx_seq2seq_generate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
+                         const int64_t* d_attention_mask, int32_t batch, int32_t in_len, int32_t num_beams,
+                         int32_t num_return, int32_t max_length, double length_penalty, int32_t eos_id,
+                         int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                         const rpx_generate_trace* trace, void* d_workspace, size_t workspace_bytes, void* stream) {
+  RPX_REQUIRE(dec && enc && d_input_ids && d_sequences && h_out_len && d_workspace, RPX_ERR_INVALID,
+              "rpx_seq2seq_generate: null argument");
+  RPX_TRY(check_pair(dec, enc));
+  const rpx_t5_config& c = dec->cfg;
+  const int V = c.vocab_size;
+  RPX_REQUIRE(batch > 0 && in_len > 0, RPX_ERR_INVALID, "rpx_seq2seq_generate: batch=%d in_len=%d", batch, in_len);
+  RPX_REQUIRE(num_beams >= 1 && num_beams <= kMaxBeams, RPX_ERR_INVALID,
+              "rpx_seq2seq_generate: num_beams=%d outside [1, %d]", num_beams, kMaxBeams);
+  RPX_REQUIRE(num_return >= 1 && num_return <= num_beams, RPX_ERR_INVALID,
+              "rpx_seq2seq_generate: num_return=%d outside [1, num_beams=%d]", num_return, num_beams);
+  RPX_REQUIRE(num_beams == 1 || 2 * num_beams <= V, RPX_ERR_INVALID,
+              "rpx_seq2seq_generate: 2 * num_beams=%d exceeds vocab_size=%d", 2 * num_beams, V);
+  RPX_REQUIRE(num_beams == 1 || d_scores, RPX_ERR_INVALID, "rpx_seq2seq_generate: beam search needs d_scores");
+  RPX_REQUIRE(max_length >= 2, RPX_ERR_INVALID, "rpx_seq2seq_generate: max_length=%d must be at least 2", max_length);
+  RPX_REQUIRE(eos_id >= 0 && eos_id < V, RPX_ERR_INVALID, "rpx_seq2seq_generate: eos_id=%d outside [0, %d)", eos_id, V);
+  RPX_REQUIRE(num_beams == 1 || beam_step_smem_bytes(num_beams, V) <= kMaxStepSmem, RPX_ERR_UNSUPPORTED,
+              "rpx_seq2seq_generate: num_beams * vocab_size=%d candidates exceed one CTA's shared memory",
+              num_beams * V);
+  RPX_REQUIRE(batch <= 65535 && (int64_t)batch * in_len < (int64_t)INT32_MAX &&
+                  (int64_t)batch * num_beams * max_length < (int64_t)INT32_MAX,
+              RPX_ERR_UNSUPPORTED, "rpx_seq2seq_generate: batch too large");
+  RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
+  RPX_REQUIRE(!trace || (trace->d_scores && trace->d_parents && trace->d_tokens && trace->max_steps >= 0),
+              RPX_ERR_INVALID, "rpx_seq2seq_generate: incomplete trace");
+  const int B = batch, nb = num_beams, R = B * nb, ML = max_length, D = c.d_model;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* base = static_cast<uint8_t*>(d_workspace);
+  const GenWs g = carve_gen(dec, enc, base, B, in_len, nb, ML);
+  RPX_REQUIRE(g.total <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu", g.total,
+              workspace_bytes);
+  if (!dec->h_poll) {
+    RPX_TRY(configure_search_step(kMaxStepSmem));
+    RPX_CUDA_OK(cudaHostAlloc(reinterpret_cast<void**>(&dec->h_poll), 32, cudaHostAllocDefault));
+    for (cudaEvent_t& ev : dec->poll_ev) RPX_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  }
+  const Workspace e_max = carve(enc, base + g.enc_off, (int64_t)B * in_len, B);
+
+  // ---- the states' lengths
+  RPX_CUDA_OK(cudaMemsetAsync(e_max.flag, 0, 4, st));
+  auto& h = dec->h_lens;
+  h.assign((size_t)B + 1, in_len);
+  h[B] = 0;
+  if (d_attention_mask) {
+    RPX_TRY(launch_mask_lengths(d_attention_mask, e_max.lens, e_max.flag, B, in_len, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(h.data(), e_max.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(&h[B], e_max.flag, 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaStreamSynchronize(st));
+    RPX_REQUIRE(h[B] == 0, RPX_ERR_MASK,
+                "attention_mask must be a right-padded prefix of ones with at least one token per row");
+  }
+  auto& cu = dec->h_cu;  // [0, B]: encoder offsets, [B + 1, 2B + 1]: the beams' query offsets (b nb)
+  cu.assign(2 * (size_t)B + 2, 0);
+  int max_enc = 0;
+  for (int b = 0; b < B; ++b) {
+    cu[b + 1] = cu[b] + h[b];
+    cu[B + 2 + b] = (b + 1) * nb;
+    max_enc = h[b] > max_enc ? h[b] : max_enc;
+  }
+  const int T_enc = cu[B];
+  const Workspace ew = carve(enc, base + g.enc_off, T_enc, B);
+  const Workspace dw = carve(enc, base + g.dec_off, R, B);
+  RPX_CUDA_OK(cudaMemcpyAsync(ew.cu_tokens, cu.data(), ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, cu.data() + B + 1, ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
+  RPX_TRY(launch_pack_ids(d_input_ids, ew.cu_tokens, ew.ids, B, in_len, T_enc, V, ew.flag, st));
+  // the host vectors stay untouched until the next call, which synchronises before reusing them
+  GenerateInitArgs ia{g.tokens, nb > 1 ? g.lin : nullptr, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.state,
+                      g.counters, g.counters + 1, g.counters + 2, R, nb > 1 ? B : R, nb, ML, dec->start_id};
+  RPX_TRY(launch_generate_init(ia, st));
+
+  // ---- prefill: encoder, then the cross K / V of every decoder layer, once per state
+  RPX_TRY(forward(enc, ew, T_enc, B, max_enc, OutKind::kResidual, 0, nullptr, 0, st));
+  {
+    PdlScope pdl_scope(T_enc <= kPdlMaxTokens);
+    RPX_TRY(qkv_gemm(false, T_enc, ew.h16, dec->cross_kv, dec->n_kv, D,
+                     RowScale{ew.ssA, enc->n_parts, T_enc, 1.0f / (float)D, c.ln_eps}, g.cross_kv, nullptr, 0, st));
+  }
+
+  // ---- the steps, enqueued in blocks; the done-state count of the block before is read while a block runs
+  const int states = nb > 1 ? B : R;
+  int t = 0, blk = 0;
+  {
+    PdlScope pdl_scope(true);
+    while (t <= ML - 2) {
+      const int t_end = t + kPollSteps < ML - 1 ? t + kPollSteps : ML - 1;
+      for (; t < t_end; ++t) {
+        RPX_TRY(decode_step(dec, enc, g, dw, ew.cu_tokens, T_enc, B, nb, ML, t, st));
+        const bool tr = trace && t < trace->max_steps;
+        BeamStepArgs sa{g.logits, g.tokens, g.lin, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.fin_seq, g.state,
+                        g.counters, g.counters + 2, tr ? trace->d_scores + (size_t)t * R * V : nullptr,
+                        tr ? trace->d_parents + (size_t)t * R : nullptr, tr ? trace->d_tokens + (size_t)t * R : nullptr,
+                        (float)pow((double)(t + 1), length_penalty), t, R, nb, V, ML, eos_id};
+        RPX_TRY(launch_search_step(sa, states, st));
+      }
+      RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + (blk & 1), g.counters, 4, cudaMemcpyDeviceToHost, st));
+      RPX_CUDA_OK(cudaEventRecord(dec->poll_ev[blk & 1], st));
+      if (blk > 0) {
+        RPX_CUDA_OK(cudaEventSynchronize(dec->poll_ev[(blk - 1) & 1]));
+        if (dec->h_poll[(blk - 1) & 1] == states) break;
+      }
+      ++blk;
+    }
+  }
+  GenerateFinishArgs fa{g.tokens, g.fin_score, g.fin_len, g.fin_seq, g.state, d_sequences, d_scores, g.counters + 1, R,
+                        nb, num_return, ML, dec->start_id, nb > 1 && dec->start_id == 0 ? eos_id : dec->start_id};
+  RPX_TRY(launch_generate_finish(fa, nb > 1 ? B : R, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 2, g.counters + 1, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 3, ew.flag, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 4, g.counters + 2, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaStreamSynchronize(st));
+  // ids outside [0, vocab) are reported after the fact (the search ran with id 0 in their place)
+  RPX_REQUIRE((dec->h_poll[3] & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", V);
+  *h_out_len = dec->h_poll[2];
+  if (h_steps) *h_steps = dec->h_poll[4];
+  return RPX_OK;
+}
+
+int rpx_debug_decode_attention(const void* d_cache, const int32_t* d_lin, const float* d_lut, void* d_out, int32_t t,
+                               int32_t rows, int32_t max_length, int32_t n_heads, int32_t rel_max_distance,
+                               void* stream) {
+  RPX_REQUIRE(d_cache && d_lut && d_out, RPX_ERR_INVALID, "rpx_debug_decode_attention: null argument");
+  RPX_REQUIRE(rows > 0 && n_heads > 0 && t >= 0 && t < max_length, RPX_ERR_INVALID,
+              "rpx_debug_decode_attention: t=%d rows=%d max_length=%d n_heads=%d", t, rows, max_length, n_heads);
+  RPX_REQUIRE(rows <= INT32_MAX / max_length, RPX_ERR_UNSUPPORTED, "rpx_debug_decode_attention: rows=%d too many", rows);
+  RPX_REQUIRE(rel_max_distance > 0 && rel_max_distance <= 2048, RPX_ERR_INVALID,
+              "rpx_debug_decode_attention: rel_max_distance=%d", rel_max_distance);
+  const int inner = n_heads * 64;
+  DecodeAttnArgs a{static_cast<const __nv_bfloat16*>(d_cache), d_lin, d_lut, static_cast<__nv_bfloat16*>(d_out), nullptr,
+                   t, rows, 3 * inner, inner, n_heads, max_length, rel_max_distance, 1};
+  return launch_decode_attention(a, static_cast<cudaStream_t>(stream));
 }
 
 int rpx_debug_attention_ex(int32_t mode, const void* d_q, const void* d_kv, void* d_out, const int32_t* d_cu_q,

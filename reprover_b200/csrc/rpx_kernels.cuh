@@ -34,6 +34,82 @@ struct AttnArgs {
 };
 int launch_t5_attention_mode(AttnMode mode, const AttnArgs& args, cudaStream_t stream);
 
+// ---- rpx_generate.cu
+// Decode self-attention: query (row r, head h) of step t against keys p = 0..t of its hypothesis.  cache: one layer,
+// [max_length][rows][ld = 3 inner] bf16 (q | k | v, head h at 64 h of each); cache row p * rows + lin[r][p] holds
+// position p of row r's hypothesis (lin [rows][max_length] int32; null: the row's own slot r at every position).
+// Score q.k (unscaled) + lut[h][max(p - t, -max_distance) + max_distance]; out [rows, inner] bf16.
+// Rows of a state with state_done[4 (r / beams)] != 0 are not written (state_done: BeamStepArgs::state, or null).
+struct DecodeAttnArgs {
+  const __nv_bfloat16* cache;
+  const int32_t* lin;
+  const float* lut;
+  __nv_bfloat16* out;
+  const int32_t* state_done;  // [states][4], word 0 = done (BeamStepArgs::state), or null
+  int t, rows, ld, inner, n_heads, max_length, max_distance, beams;
+};
+int launch_decode_attention(const DecodeAttnArgs& a, cudaStream_t stream);
+
+// One search step over fp32 logits [rows, vocab], rows = states * beams (rpx_generate.cu documents the rules).
+// tokens [max_length][rows]: the input token of every row at every step (step t + 1's are written here).
+// state [states][4]: done, early-stop heuristic unsatisfied, finished-buffer parity, unused.
+// Finished hypotheses (beams > 1): [2][rows] scores / lengths / flags, [2][rows][max_length] generated tokens.
+// Greedy (beams == 1) keeps each row's generated length in fin_len[r].  trace_*: this step's log-probs (greedy:
+// logits) [rows, vocab], parents (global row) and tokens [rows] of the next step's running rows, or null.
+struct BeamStepArgs {
+  const float* logits;
+  int32_t* tokens;
+  int32_t* lin;  // [2][rows][max_length], parity t & 1 is step t's
+  float* run_score;
+  float* fin_score;
+  int32_t* fin_len;
+  int32_t* fin_flag;
+  int32_t* fin_seq;
+  int32_t* state;
+  int32_t* done_count;
+  int32_t* last_step;  // max over states of (step at which the state's search ended) + 1: the steps HF runs
+  float* trace_scores;
+  int32_t* trace_parents;
+  int32_t* trace_tokens;
+  float penalty;  // (float)((t + 1) ** length_penalty), computed in double as Python does
+  int t, rows, beams, vocab, max_length, eos;
+};
+// Dynamic shared memory of one beam step CTA (the beams * vocab candidate keys).
+size_t beam_step_smem_bytes(int beams, int vocab);
+// Allows the beam step kernel up to max_smem bytes of dynamic shared memory on the current device (once per decoder).
+int configure_search_step(size_t max_smem);
+int launch_search_step(const BeamStepArgs& a, int states, cudaStream_t stream);
+
+struct GenerateInitArgs {
+  int32_t* tokens;
+  int32_t* lin;  // null for greedy
+  float* run_score;
+  float* fin_score;
+  int32_t* fin_len;
+  int32_t* fin_flag;
+  int32_t* state;
+  int32_t* done_count;
+  int32_t* out_len;
+  int32_t* last_step;
+  int rows, states, beams, max_length, start_id;
+};
+int launch_generate_init(const GenerateInitArgs& a, cudaStream_t stream);
+
+// sequences [states * n_ret, max_length] int64: start id, the generated tokens, fill_id after them; scores
+// [states * n_ret] (beams > 1); out_len = 1 + the longest returned hypothesis.
+struct GenerateFinishArgs {
+  const int32_t* tokens;
+  const float* fin_score;
+  const int32_t* fin_len;
+  const int32_t* fin_seq;
+  const int32_t* state;
+  int64_t* sequences;
+  float* scores;
+  int32_t* out_len;
+  int rows, beams, n_ret, max_length, start_id, fill_id;
+};
+int launch_generate_finish(const GenerateFinishArgs& a, int states, cudaStream_t stream);
+
 // ---- rpx_elementwise.cu
 // ByT5 tokenisation of packed byte strings into packed token ids (byte + 3, EOS = 1 last,
 // truncated to max_seq_len including EOS).  cu_bytes / cu_tokens are [n_seqs + 1] device arrays.

@@ -7,17 +7,21 @@ retriever's `self.encoder`.  Called as the reference calls it in `forward` (gene
     gen(input_ids=state_ids, attention_mask=state_mask, labels=tactic_ids).loss
 
 it returns HF's loss, the logits and the per-row log-likelihoods of the labels, all computed by `rpx_seq2seq_forward`
-(encoder, cross K / V, decoder layers, head and log-softmax in sm_90a CUDA).  Beam search / `generate` is not here.
+(encoder, cross K / V, decoder layers, head and log-softmax in sm_90a CUDA).  `generate` runs HF's beam search
+(or greedy search) over an incremental decoder with a KV cache (`rpx_seq2seq_generate`), as the reference calls it in
+`HuggingFaceGenerator.generate` (prover/tactic_generator.py) and `validation_step` (generation/model.py).
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, NamedTuple, Optional, Union
+import json
+import os
+from typing import Any, Dict, NamedTuple, Optional, Union
 
 import torch
 
 from . import _native
-from .engine import EncoderConfig, T5EncoderEngine, _stream_ptr, load_hf_checkpoint
+from .engine import EncoderConfig, T5EncoderEngine, _stream_ptr, load_hf_checkpoint, resolve_checkpoint_dir
 
 _DEC_LAYER_KEYS = {
     "h_q": "decoder.block.{i}.layer.0.SelfAttention.q.weight",
@@ -89,6 +93,113 @@ def check_generator_checkpoint(config: Dict, state_dict: Dict[str, torch.Tensor]
     return g
 
 
+# HF `GenerationConfig` defaults of the settings `generate` reads (transformers 5.5)
+GENERATION_DEFAULTS = {"max_length": 20, "num_beams": 1, "num_return_sequences": 1, "length_penalty": 1.0,
+                       "early_stopping": False, "do_sample": False}
+# Settings whose value, other than the one listed, makes HF add a logits processor, a stopping criterion or a
+# decoding mode the engine does not run.
+_NEUTRAL = {"min_length": 0, "min_new_tokens": None, "max_new_tokens": None, "no_repeat_ngram_size": 0,
+            "encoder_no_repeat_ngram_size": 0, "repetition_penalty": 1.0, "encoder_repetition_penalty": 1.0,
+            "bad_words_ids": None, "force_words_ids": None, "forced_bos_token_id": None, "forced_eos_token_id": None,
+            "suppress_tokens": None, "begin_suppress_tokens": None, "sequence_bias": None,
+            "exponential_decay_length_penalty": None, "renormalize_logits": False, "num_beam_groups": 1,
+            "diversity_penalty": 0.0, "constraints": None, "max_time": None, "stop_strings": None,
+            "logits_processor": None, "stopping_criteria": None, "prefix_allowed_tokens_fn": None,
+            "guidance_scale": None, "low_memory": None, "output_attentions": False, "output_hidden_states": False,
+            "output_logits": False, "assistant_model": None, "streamer": None, "synced_gpus": None,
+            "decoder_input_ids": None, "use_cache": True, "watermarking_config": None, "epsilon_cutoff": 0.0,
+            "eta_cutoff": 0.0}
+# Sampling settings: HF ignores them when do_sample is False, and so does the engine.
+_IGNORED = {"temperature", "top_k", "top_p", "min_p", "typical_p", "top_h"}
+
+
+class GenerationSettings(NamedTuple):
+    """What `generation_settings` decides for one `generate` call."""
+
+    max_length: int
+    num_beams: int
+    num_return_sequences: int
+    length_penalty: float
+    eos_token_id: int
+    pad_token_id: int
+    decoder_start_token_id: int
+    output_scores: bool
+    return_dict_in_generate: bool
+
+
+def generation_settings(config: Dict, generation_config: Optional[Dict] = None, **kwargs: Any) -> GenerationSettings:
+    """HF `generate`'s settings as the engine runs them: a keyword argument wins over the checkpoint's
+    `generation_config.json` (`generation_config`), which wins over HF's `GenerationConfig` defaults.  `eos_token_id`,
+    `pad_token_id` and `decoder_start_token_id` come from the same chain, ending at the model config.
+    Raises NotImplementedError naming each setting the engine does not run: `do_sample=True`, `early_stopping` other
+    than False, `max_new_tokens`, a list of EOS ids, and any setting that would make HF add a logits processor or a
+    stopping criterion (`min_length`, `no_repeat_ngram_size`, `repetition_penalty`, `bad_words_ids`, ...)."""
+    gen = dict(generation_config or {})
+    given = {k: v for k, v in kwargs.items() if v is not None}
+
+    def pick(name, fallback=None):
+        if name in given:
+            return given[name]
+        if gen.get(name) is not None:
+            return gen[name]
+        if name in GENERATION_DEFAULTS:
+            return GENERATION_DEFAULTS[name]
+        return config.get(name, fallback)
+
+    refused = []
+    if bool(pick("do_sample")):
+        refused.append("do_sample=True")
+    if pick("early_stopping") is not False:
+        refused.append(f"early_stopping={pick('early_stopping')!r}")
+    known = set(GENERATION_DEFAULTS) | {"eos_token_id", "pad_token_id", "decoder_start_token_id", "output_scores",
+                                        "return_dict_in_generate"}
+    for source in (gen, given):
+        for name, value in source.items():
+            if name in known or name in _IGNORED or value is None:
+                continue
+            if name not in _NEUTRAL:
+                if source is given:
+                    refused.append(name)
+                continue
+            if value != _NEUTRAL[name] and f"{name}={value!r}" not in refused:
+                refused.append(f"{name}={value!r}")
+    eos = pick("eos_token_id")
+    if isinstance(eos, (list, tuple)):
+        if len(eos) != 1:
+            refused.append(f"eos_token_id={list(eos)!r} (one EOS id only)")
+        else:
+            eos = eos[0]
+    if eos is None:
+        refused.append("eos_token_id=None (the engine stops on one EOS id)")
+    if refused:
+        raise NotImplementedError(f"T5GeneratorEngine.generate runs beam or greedy search with one EOS id and no "
+                                  f"logits processor; not supported: {refused}")
+    num_beams = int(pick("num_beams"))
+    n_ret = int(pick("num_return_sequences"))
+    max_length = int(pick("max_length"))
+    if num_beams < 1:
+        raise ValueError(f"num_beams={num_beams} must be at least 1")
+    if not 1 <= n_ret <= num_beams:
+        raise ValueError(f"num_return_sequences={n_ret} must be in [1, num_beams={num_beams}]")
+    if max_length < 2:
+        raise ValueError(f"max_length={max_length}: the engine generates at least one token after the start token")
+    pad = int(pick("pad_token_id", 0))
+    start = pick("decoder_start_token_id")
+    start = pad if start is None else int(start)
+    return GenerationSettings(max_length, num_beams, n_ret, float(pick("length_penalty")), int(eos), pad, start,
+                              bool(kwargs.get("output_scores") or gen.get("output_scores") or False),
+                              bool(kwargs.get("return_dict_in_generate") or gen.get("return_dict_in_generate")
+                                   or False))
+
+
+class GenerateOutput(NamedTuple):
+    """HF `generate(..., return_dict_in_generate=True)`'s output as far as the reference reads it.  The per-step
+    `.scores` tuple is not produced."""
+
+    sequences: torch.Tensor                   # int64 [B * num_return_sequences, L_out], state-major, best first
+    sequences_scores: Optional[torch.Tensor]  # fp32 [B * num_return_sequences]; None for greedy or without output_scores
+
+
 class Seq2SeqOutput(NamedTuple):
     """What HF `T5ForConditionalGeneration` returns, as far as the reference reads it (`.loss`, `.logits`), plus
     the per-row sums the loss is made of."""
@@ -102,8 +213,10 @@ class Seq2SeqOutput(NamedTuple):
 class T5GeneratorEngine:
     """ByT5/T5 encoder-decoder, teacher-forced, on one GPU (`rpx_seq2seq_forward`)."""
 
-    def __init__(self, config: Dict, state_dict: Dict[str, torch.Tensor], device: Union[int, str, torch.device]) -> None:
+    def __init__(self, config: Dict, state_dict: Dict[str, torch.Tensor], device: Union[int, str, torch.device],
+                 generation_config: Optional[Dict] = None) -> None:
         g = check_generator_checkpoint(config, state_dict)
+        self.generation_config = dict(generation_config or {})
         self.lib = _native.load()
         self.device = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
         if self.device.type != "cuda":
@@ -154,6 +267,10 @@ class T5GeneratorEngine:
     @classmethod
     def from_hf_dir(cls, path: str, device, **kw) -> "T5GeneratorEngine":
         cfg, sd = load_hf_checkpoint(path)
+        gc_path = os.path.join(resolve_checkpoint_dir(path), "generation_config.json")
+        if "generation_config" not in kw and os.path.exists(gc_path):
+            with open(gc_path) as fh:
+                kw["generation_config"] = json.load(fh)
         return cls(cfg, sd, device, **kw)
 
     def close(self) -> None:
@@ -230,3 +347,89 @@ class T5GeneratorEngine:
         return Seq2SeqOutput(loss, logits, seq_lp, seq_n)
 
     forward = __call__
+
+    def to(self, device=None, *args: Any, **kwargs: Any) -> "T5GeneratorEngine":
+        """HF's `model.to(device)`, as the reference calls it after loading a generator: the engine is bound to the
+        GPU it was built on, so this returns it unchanged for that device (or no device) and raises for another."""
+        if device is not None and not isinstance(device, torch.dtype):
+            d = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
+            same = d.type == "cuda" and (d.index is None or d.index == self.device.index
+                                         or (self.device.index is None and d.index == torch.cuda.current_device()))
+            if not same:
+                raise ValueError(f"T5GeneratorEngine lives on {self.device}; it cannot move to {d}")
+        return self
+
+    def eval(self) -> "T5GeneratorEngine":
+        """HF's `model.eval()`: the engine only evaluates, so it is returned unchanged."""
+        return self
+
+    def generate(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor] = None, *,
+                 max_length: Optional[int] = None, num_beams: Optional[int] = None, do_sample: Optional[bool] = None,
+                 num_return_sequences: Optional[int] = None, length_penalty: Optional[float] = None,
+                 early_stopping: Optional[Union[bool, str]] = None, output_scores: bool = False,
+                 return_dict_in_generate: bool = False, _trace_steps: int = 0, **unsupported: Any):
+        """HF `T5ForConditionalGeneration.generate` for beam search (`num_beams > 1`) and greedy search, as the
+        reference calls it.  Returns the sequences [B * num_return_sequences, L_out] (int64, on the engine's device),
+        or with `return_dict_in_generate` a `GenerateOutput` with `.sequences` and `.sequences_scores` (None for greedy
+        or without `output_scores`, as HF).  Settings follow `generation_settings`; a `pad_token_id` other than the
+        decoder start id is refused (the engine fills with the start id, or EOS when that is 0, as HF's
+        `output_fill_value` does for T5).  `_trace_steps` (tests) records each of the first that many steps and returns
+        `(output, trace)`: "scores" [steps, R, V] (log-probs; logits for greedy), "parents" and "tokens" [steps, R],
+        and "steps", the decoder steps HF runs for this call (the step at which the last search ended)."""
+        s = generation_settings(self.config, self.generation_config, max_length=max_length, num_beams=num_beams,
+                                do_sample=do_sample, num_return_sequences=num_return_sequences,
+                                length_penalty=length_penalty, early_stopping=early_stopping,
+                                output_scores=output_scores, return_dict_in_generate=return_dict_in_generate,
+                                **unsupported)
+        if s.decoder_start_token_id != self.gen_config.start_token_id:
+            raise NotImplementedError(f"decoder_start_token_id={s.decoder_start_token_id}: the engine starts every "
+                                      f"hypothesis with the config's {self.gen_config.start_token_id}")
+        if s.pad_token_id != self.gen_config.start_token_id:
+            raise NotImplementedError(f"pad_token_id={s.pad_token_id}: the engine pads with the decoder start id "
+                                      f"{self.gen_config.start_token_id}, as `_shift_right` does")
+        if input_ids is None or input_ids.dim() != 2:
+            raise ValueError("input_ids must be a [batch, seq_len] tensor")
+        ids = input_ids.to(device=self.device, dtype=torch.int64).contiguous()
+        mask = None
+        if attention_mask is not None:
+            if attention_mask.shape != input_ids.shape:
+                raise ValueError(f"attention_mask {tuple(attention_mask.shape)} != input_ids {tuple(input_ids.shape)}")
+            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
+        seqs, scores, trace = self._search(ids, mask, s, int(_trace_steps))
+        if not s.return_dict_in_generate:
+            if trace is not None:
+                return GenerateOutput(seqs, scores), trace
+            return seqs
+        out = GenerateOutput(seqs, scores if s.output_scores else None)
+        return (out, trace) if trace is not None else out
+
+    def _search(self, ids: torch.Tensor, mask: Optional[torch.Tensor], s: GenerationSettings, trace_steps: int):
+        """rpx_seq2seq_generate on device ids / mask: (sequences [B * n_ret, L_out], scores or None, trace or None)."""
+        B, L_in = ids.shape
+        nb, n_ret, ML = s.num_beams, s.num_return_sequences, s.max_length
+        R = B * nb
+        seqs = torch.empty(B * n_ret, ML, dtype=torch.int64, device=self.device)
+        scores = torch.empty(B * n_ret, dtype=torch.float32, device=self.device) if nb > 1 else None
+        trace = None
+        if trace_steps:
+            n = min(trace_steps, ML - 1)
+            trace = {"scores": torch.full((n, R, self.vocab_size), float("nan"), device=self.device),
+                     "parents": torch.full((n, R), -1, dtype=torch.int32, device=self.device),
+                     "tokens": torch.full((n, R), -1, dtype=torch.int32, device=self.device)}
+            c_trace = _native.GenerateTrace(trace["scores"].data_ptr(), trace["parents"].data_ptr(),
+                                            trace["tokens"].data_ptr(), n)
+        out_len, steps = C.c_int32(0), C.c_int32(0)
+        with torch.cuda.device(self.device):
+            need = self.lib.rpx_seq2seq_generate_workspace_bytes(self._handle, self.encoder._handle, B, L_in, nb, ML)
+            if need == 0:
+                raise _native.RpxError(_native.RPX_ERR_INVALID, f"no generate workspace for batch={B} in_len={L_in} "
+                                       f"num_beams={nb} max_length={ML}")
+            ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            _native.check(self.lib.rpx_seq2seq_generate(
+                self._handle, self.encoder._handle, ids.data_ptr(), None if mask is None else mask.data_ptr(), B, L_in,
+                nb, n_ret, ML, s.length_penalty, s.eos_token_id, seqs.data_ptr(),
+                None if scores is None else scores.data_ptr(), C.byref(out_len), C.byref(steps),
+                None if trace is None else C.byref(c_trace), ws.data_ptr(), ws.numel(), _stream_ptr(self.device)))
+        if trace is not None:
+            trace["steps"] = steps.value
+        return seqs[:, :out_len.value].contiguous(), scores, trace
