@@ -291,6 +291,21 @@ int rpx_seq2seq_generate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d
                          int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
                          const rpx_generate_trace* trace, void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* Workspace of one rpx_seq2seq_evaluate call (0 when the arguments are out of range or `dec` and `enc` do not fit
+ * together): one prefill, and the larger of the two halves' own regions, which they share. */
+size_t rpx_seq2seq_evaluate_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch,
+                                            int32_t in_len, int32_t out_len, int32_t num_beams, int32_t max_length);
+/* rpx_seq2seq_forward and rpx_seq2seq_generate on the same states, as the reference's `validation_step` runs the loss
+ * and `generate` on one batch, with the encoder and the cross K / V computed once for both.  Every argument means what
+ * it means in those two calls, and each output equals theirs bit for bit.  The checks are those of both calls; the
+ * label check comes before anything runs, the id check once after both halves.  Synchronises `stream`. */
+int rpx_seq2seq_evaluate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
+                         const int64_t* d_attention_mask, int32_t batch, int32_t in_len, const int64_t* d_labels,
+                         int32_t out_len, float* d_logits, double* d_seq_logprob, int32_t* d_seq_count,
+                         int32_t num_beams, int32_t num_return, int32_t max_length, double length_penalty,
+                         int32_t eos_id, int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                         void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* --------------------------------------------------------------- similarity + top-k
  * Replaces the matmul + argsort half of `Corpus.get_nearest_premises`
  * (common.py:307-308) and the first-k walk at :316-322:

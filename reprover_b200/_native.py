@@ -138,6 +138,12 @@ _SIGNATURES = {
                                        C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p,
                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_size_t,
                                        C.c_void_p]),
+    "rpx_seq2seq_evaluate_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                                          C.c_int32, C.c_int32]),
+    "rpx_seq2seq_evaluate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
+                                       C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_debug_decode_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                              C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "rpx_encoder_set_debug_hidden": (C.c_int, [C.c_void_p, C.c_void_p]),

@@ -64,6 +64,25 @@ def remove_marks(s: str) -> str:
     return s.replace(MARK_START_SYMBOL, "").replace(MARK_END_SYMBOL, "")
 
 
+def format_augmented_state(s: str, premises: Sequence["Premise"], max_len: Optional[int] = None) -> str:
+    """The reference's `format_augmented_state` (common.py) without `p_drop`, which only training sets: the state
+    with retrieved premises prepended, each as `p.serialize() + "\n\n"`.  Lengths are UTF-8 bytes; the premises'
+    budget is `max_len` minus the state's length (it may be negative).  A premise that would overrun the budget is
+    skipped, and later, shorter ones may still fit.  Each accepted premise goes in front of the text so far, so the
+    top-ranked premise ends up farthest from the state.  `max_len=None`: no budget."""
+    budget = None if max_len is None else max_len - len(s.encode("utf-8"))
+    aug = ""
+    length = 0
+    for p in premises:
+        p_str = f"{p.serialize()}\n\n"
+        n = len(p_str.encode("utf-8"))
+        if budget is not None and length + n > budget:
+            continue
+        length += n
+        aug = p_str + aug
+    return aug + s
+
+
 @dataclass(unsafe_hash=True)
 class Context:
     """A retrieval query: a proof state inside a theorem (reference common.py:34-56)."""

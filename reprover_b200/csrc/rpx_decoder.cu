@@ -15,6 +15,10 @@
 //              their sum in token order.
 // Row b's decoder tokens are positions [0, len_b) with len_b = 1 + the last position whose label is not -100; the
 // positions past it are never computed.
+//
+// The encoder and the cross K / V are the prefill that rpx_seq2seq_forward, rpx_seq2seq_generate and
+// rpx_seq2seq_evaluate share (`prefill` below); evaluate runs it once and hands it to both the teacher-forced half and
+// the search, as the reference's `validation_step` needs both on one batch.
 #include <math.h>
 
 #include <new>
@@ -221,37 +225,56 @@ __global__ void scatter_logits_kernel(const float* __restrict__ packed, const in
   for (int c = lane; c < n4; c += 32) dst[c] = src[c];
 }
 
-// Device buffers of one call: the encoder's workspace, the decoder's (same members, for the decoder tokens), and
-// the generator's own.  Every region is sized for the worst case (all positions tokens), so none moves with the
-// actual token counts; within the two forward workspaces, carve() keeps the S-sized members in place.
-struct SeqWs {
-  size_t enc_off, dec_off;
+// Device buffers of one call.  Every region is sized for the worst case (all positions tokens), so none moves with
+// the actual token counts; within the forward workspaces, carve() keeps the S-sized members in place.  The prefill's
+// regions (the encoder's workspace and the cross K / V) come first; each half carves its own regions after them, from
+// `base` on.  Each carve_* sizes only when `base` is null.
+struct PrefillWs {
+  size_t enc_off;
   __nv_bfloat16* cross_kv;  // [B * in_len, n_kv]
+  size_t total;
+};
+
+// The teacher-forced half: the decoder's workspace (the encoder's members, for the decoder tokens) and its own.
+struct SeqWs {
+  size_t dec_off;
   float* logits;            // [B * out_len, vocab]
   double* tok_lp;           // [B * out_len]
   int32_t* targets;         // [B * out_len]
   size_t total;
 };
 
-SeqWs carve_seq(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, int64_t B, int64_t in_len,
-                int64_t out_len) {
-  SeqWs w{};
-  const int64_t Te = B * in_len, Td = B * out_len;
+struct Carver {
+  uint8_t* base;
   size_t off = 0;
-  auto take = [&](size_t bytes) {
+  uint8_t* take(size_t bytes) {
     uint8_t* p = base ? base + off : nullptr;
     off = align_up(off + bytes, 256);
     return p;
-  };
-  w.enc_off = off;
-  take(carve(e, nullptr, Te, B).total);
-  w.dec_off = off;
-  take(carve(e, nullptr, Td, B).total);
-  w.cross_kv = (__nv_bfloat16*)take((size_t)Te * d->n_kv * 2);
-  w.logits = (float*)take((size_t)Td * d->cfg.vocab_size * 4);
-  w.tok_lp = (double*)take((size_t)Td * 8);
-  w.targets = (int32_t*)take((size_t)Td * 4);
-  w.total = off;
+  }
+};
+
+PrefillWs carve_prefill(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, int64_t B, int64_t in_len) {
+  PrefillWs w{};
+  const int64_t Te = B * in_len;
+  Carver c{base};
+  w.enc_off = c.off;
+  c.take(carve(e, nullptr, Te, B).total);
+  w.cross_kv = (__nv_bfloat16*)c.take((size_t)Te * d->n_kv * 2);
+  w.total = c.off;
+  return w;
+}
+
+SeqWs carve_seq(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, int64_t B, int64_t out_len) {
+  SeqWs w{};
+  const int64_t Td = B * out_len;
+  Carver c{base};
+  w.dec_off = c.off;
+  c.take(carve(e, nullptr, Td, B).total);
+  w.logits = (float*)c.take((size_t)Td * d->cfg.vocab_size * 4);
+  w.tok_lp = (double*)c.take((size_t)Td * 8);
+  w.targets = (int32_t*)c.take((size_t)Td * 4);
+  w.total = c.off;
   return w;
 }
 
@@ -292,11 +315,11 @@ int decoder_layer(const rpx_t5_decoder* d, const DecLayerW& w, int layer, const 
 }
 
 // ---------------------------------------------------------------------------------------------- generate
-// Device buffers of one generate call over B states, nb beams, R = B nb rows.  Nothing here grows with the step:
-// the KV cache holds every step's q | k | v rows in place, [num_layers][max_length][R][3 inner] bf16.
+// The search half over B states, nb beams, R = B nb rows.  Nothing here grows with the step: the KV cache holds
+// every step's q | k | v rows in place, [num_layers][max_length][R][3 inner] bf16.
 struct GenWs {
-  size_t enc_off, dec_off;
-  __nv_bfloat16* cross_kv;  // [B * in_len, n_kv]
+  size_t dec_off;
+  __nv_bfloat16* cross_kv;  // the prefill's
   __nv_bfloat16* cache;
   float* logits;            // [R, vocab]
   int32_t* tokens;          // [max_length][R]
@@ -312,34 +335,27 @@ struct GenWs {
   size_t total;
 };
 
-GenWs carve_gen(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, int64_t B, int64_t in_len, int64_t nb,
-                int64_t ML) {
+GenWs carve_gen(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, __nv_bfloat16* cross_kv, int64_t B,
+                int64_t nb, int64_t ML) {
   GenWs w{};
-  const int64_t Te = B * in_len, R = B * nb;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    uint8_t* p = base ? base + off : nullptr;
-    off = align_up(off + bytes, 256);
-    return p;
-  };
-  w.enc_off = off;
-  take(carve(e, nullptr, Te, B).total);
-  w.dec_off = off;
-  take(carve(e, nullptr, R, B).total);
-  w.cross_kv = (__nv_bfloat16*)take((size_t)Te * d->n_kv * 2);
+  const int64_t R = B * nb;
+  Carver c{base};
+  w.dec_off = c.off;
+  c.take(carve(e, nullptr, R, B).total);
+  w.cross_kv = cross_kv;
   w.cache_layer = (size_t)ML * R * 3 * d->inner;
-  w.cache = (__nv_bfloat16*)take(w.cache_layer * d->cfg.num_layers * 2);
-  w.logits = (float*)take((size_t)R * d->cfg.vocab_size * 4);
-  w.tokens = (int32_t*)take((size_t)ML * R * 4);
-  w.lin = (int32_t*)take(2 * (size_t)R * ML * 4);
-  w.run_score = (float*)take((size_t)R * 4);
-  w.fin_score = (float*)take(2 * (size_t)R * 4);
-  w.fin_len = (int32_t*)take(2 * (size_t)R * 4);
-  w.fin_flag = (int32_t*)take(2 * (size_t)R * 4);
-  w.fin_seq = (int32_t*)take(2 * (size_t)R * ML * 4);
-  w.state = (int32_t*)take((size_t)B * 16);
-  w.counters = (int32_t*)take(16);
-  w.total = off;
+  w.cache = (__nv_bfloat16*)c.take(w.cache_layer * d->cfg.num_layers * 2);
+  w.logits = (float*)c.take((size_t)R * d->cfg.vocab_size * 4);
+  w.tokens = (int32_t*)c.take((size_t)ML * R * 4);
+  w.lin = (int32_t*)c.take(2 * (size_t)R * ML * 4);
+  w.run_score = (float*)c.take((size_t)R * 4);
+  w.fin_score = (float*)c.take(2 * (size_t)R * 4);
+  w.fin_len = (int32_t*)c.take(2 * (size_t)R * 4);
+  w.fin_flag = (int32_t*)c.take(2 * (size_t)R * 4);
+  w.fin_seq = (int32_t*)c.take(2 * (size_t)R * ML * 4);
+  w.state = (int32_t*)c.take((size_t)B * 16);
+  w.counters = (int32_t*)c.take(16);
+  w.total = c.off;
   return w;
 }
 
@@ -382,6 +398,213 @@ int decode_step(const rpx_t5_decoder* d, const rpx_encoder* e, const GenWs& g, c
 constexpr int kPollSteps = 8;
 constexpr int kMaxBeams = 128;
 constexpr size_t kMaxStepSmem = 227 * 1024 - 16 * 1024;  // the beam step's candidate keys, beside its static arrays
+
+// ---------------------------------------------------------------------------------------------- the three stages
+// rpx_seq2seq_forward, _generate and _evaluate are each a sequence of these: prefill, then the teacher-forced half, the
+// search half, or both on the one prefill.
+
+// What the prefill leaves for the halves.
+struct Prefill {
+  Workspace ew;  // the encoder's workspace for T_enc tokens: cu_tokens = the states' offsets, flag = the id-range flag
+  int T_enc, max_enc;
+  int T_dec, max_dec;  // with labels: the decoder tokens and the longest row; dec->h_cu[B + 1, 2B + 1] their offsets
+};
+
+// Argument checks of the teacher-forced half.
+int check_seq_args(const char* fn, int batch, int in_len, int out_len, const float* d_logits) {
+  RPX_REQUIRE(batch > 0 && in_len > 0 && out_len > 0, RPX_ERR_INVALID, "%s: batch=%d in_len=%d out_len=%d", fn, batch,
+              in_len, out_len);
+  RPX_REQUIRE(batch <= 65535, RPX_ERR_UNSUPPORTED, "%s: batch=%d exceeds the 65535 grid limit", fn, batch);
+  RPX_REQUIRE((int64_t)batch * in_len < (int64_t)INT32_MAX && (int64_t)batch * out_len < (int64_t)INT32_MAX,
+              RPX_ERR_UNSUPPORTED, "%s: batch too large", fn);
+  RPX_REQUIRE(d_logits == nullptr || (reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, RPX_ERR_INVALID,
+              "%s: d_logits must be 16-byte aligned", fn);
+  return RPX_OK;
+}
+
+// Argument checks of the search half.
+int check_gen_args(const char* fn, int batch, int in_len, int num_beams, int num_return, int max_length, int eos_id,
+                   const float* d_scores, int V) {
+  RPX_REQUIRE(batch > 0 && in_len > 0, RPX_ERR_INVALID, "%s: batch=%d in_len=%d", fn, batch, in_len);
+  RPX_REQUIRE(num_beams >= 1 && num_beams <= kMaxBeams, RPX_ERR_INVALID, "%s: num_beams=%d outside [1, %d]", fn,
+              num_beams, kMaxBeams);
+  RPX_REQUIRE(num_return >= 1 && num_return <= num_beams, RPX_ERR_INVALID,
+              "%s: num_return=%d outside [1, num_beams=%d]", fn, num_return, num_beams);
+  RPX_REQUIRE(num_beams == 1 || 2 * num_beams <= V, RPX_ERR_INVALID, "%s: 2 * num_beams=%d exceeds vocab_size=%d", fn,
+              2 * num_beams, V);
+  RPX_REQUIRE(num_beams == 1 || d_scores, RPX_ERR_INVALID, "%s: beam search needs d_scores", fn);
+  RPX_REQUIRE(max_length >= 2, RPX_ERR_INVALID, "%s: max_length=%d must be at least 2", fn, max_length);
+  RPX_REQUIRE(eos_id >= 0 && eos_id < V, RPX_ERR_INVALID, "%s: eos_id=%d outside [0, %d)", fn, eos_id, V);
+  RPX_REQUIRE(num_beams == 1 || beam_step_smem_bytes(num_beams, V) <= kMaxStepSmem, RPX_ERR_UNSUPPORTED,
+              "%s: num_beams * vocab_size=%d candidates exceed one CTA's shared memory", fn, num_beams * V);
+  RPX_REQUIRE(batch <= 65535 && (int64_t)batch * in_len < (int64_t)INT32_MAX &&
+                  (int64_t)batch * num_beams * max_length < (int64_t)INT32_MAX,
+              RPX_ERR_UNSUPPORTED, "%s: batch too large", fn);
+  return RPX_OK;
+}
+
+// The search step's shared-memory opt-in and the pinned words the search polls, once per decoder handle.
+int init_search(rpx_t5_decoder* dec) {
+  if (dec->h_poll) return RPX_OK;
+  RPX_TRY(configure_search_step(kMaxStepSmem));
+  RPX_CUDA_OK(cudaHostAlloc(reinterpret_cast<void**>(&dec->h_poll), 32, cudaHostAllocDefault));
+  for (cudaEvent_t& ev : dec->poll_ev) RPX_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  return RPX_OK;
+}
+
+// Stage 1, the prefill.  The states' mask lengths and, with labels, the labels' lengths (into lab_lens / lab_flag)
+// are read back in one synchronisation, none without mask and labels.  Then the host offsets, the packed ids, the
+// encoder stopped before its final RMSNorm, and the cross K / V of every decoder layer into pw.cross_kv, which is
+// skipped only when there is no search and no decoder token.  Host offsets in dec->h_cu: [0, B] the states',
+// [B + 1, 2B + 1] the decoder tokens' (with labels), [2B + 2, 3B + 2] left to the search.
+int prefill(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids, const int64_t* d_attention_mask, int B,
+            int in_len, const int64_t* d_labels, int out_len, int32_t* lab_lens, int32_t* lab_flag, uint8_t* base,
+            const PrefillWs& pw, bool search, Prefill* p, cudaStream_t st) {
+  const rpx_t5_config& c = dec->cfg;
+  const int D = c.d_model, V = c.vocab_size;
+  const Workspace e_max = carve(enc, base + pw.enc_off, (int64_t)B * in_len, B);
+
+  // ---- lengths: the state mask's and the labels', read back together
+  RPX_CUDA_OK(cudaMemsetAsync(e_max.flag, 0, 4, st));
+  auto& h = dec->h_lens;  // enc lens [B], enc flag, dec lens [B], dec flag
+  h.assign(2 * (size_t)B + 2, in_len);
+  h[B] = 0;
+  h[2 * B + 1] = 0;
+  if (d_attention_mask) {
+    RPX_TRY(launch_mask_lengths(d_attention_mask, e_max.lens, e_max.flag, B, in_len, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(h.data(), e_max.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(&h[B], e_max.flag, 4, cudaMemcpyDeviceToHost, st));
+  }
+  if (d_labels) {
+    RPX_CUDA_OK(cudaMemsetAsync(lab_flag, 0, 4, st));
+    label_lengths_kernel<<<ceil_div(B, 8), 256, 0, st>>>(d_labels, lab_lens, lab_flag, B, out_len, V);
+    RPX_CUDA_OK(cudaGetLastError());
+    RPX_CUDA_OK(cudaMemcpyAsync(&h[B + 1], lab_lens, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
+    RPX_CUDA_OK(cudaMemcpyAsync(&h[2 * B + 1], lab_flag, 4, cudaMemcpyDeviceToHost, st));
+  }
+  if (d_attention_mask || d_labels) RPX_CUDA_OK(cudaStreamSynchronize(st));
+  RPX_REQUIRE(h[B] == 0, RPX_ERR_MASK,
+              "attention_mask must be a right-padded prefix of ones with at least one token per row");
+  RPX_REQUIRE(h[2 * B + 1] == 0, RPX_ERR_INVALID, "labels must be -100 or ids in [0, %d)", V);
+
+  auto& cu = dec->h_cu;
+  cu.assign(3 * (size_t)B + 3, 0);
+  p->max_enc = p->max_dec = 0;
+  for (int b = 0; b < B; ++b) {
+    cu[b + 1] = cu[b] + h[b];
+    p->max_enc = h[b] > p->max_enc ? h[b] : p->max_enc;
+    if (d_labels) {
+      cu[B + 2 + b] = cu[B + 1 + b] + h[B + 1 + b];
+      p->max_dec = h[B + 1 + b] > p->max_dec ? h[B + 1 + b] : p->max_dec;
+    }
+  }
+  p->T_enc = cu[B];
+  p->T_dec = cu[2 * B + 1];
+  p->ew = carve(enc, base + pw.enc_off, p->T_enc, B);
+  const Workspace& ew = p->ew;
+  // the host vectors stay untouched until the next call, which synchronises before reusing them
+  RPX_CUDA_OK(cudaMemcpyAsync(ew.cu_tokens, cu.data(), ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
+  RPX_TRY(launch_pack_ids(d_input_ids, ew.cu_tokens, ew.ids, B, in_len, p->T_enc, V, ew.flag, st));
+
+  // ---- encoder, then the cross K / V of every decoder layer, once per state
+  RPX_TRY(forward(enc, ew, p->T_enc, B, p->max_enc, OutKind::kResidual, 0, nullptr, 0, st));
+  if (search || p->T_dec > 0) {
+    PdlScope pdl_scope(p->T_enc <= kPdlMaxTokens && p->T_dec <= kPdlMaxTokens);
+    RPX_TRY(qkv_gemm(false, p->T_enc, ew.h16, dec->cross_kv, dec->n_kv, D,
+                     RowScale{ew.ssA, enc->n_parts, p->T_enc, 1.0f / (float)D, c.ln_eps}, pw.cross_kv, nullptr, 0,
+                     st));
+  }
+  return RPX_OK;
+}
+
+// Stage 2, the teacher-forced half: `_shift_right(labels)` through the decoder layers, the head and log-softmax; the
+// per-row sums and counts into d_seq_logprob / d_seq_count, the logits into d_logits unless it is null.
+int teacher_forced(const rpx_t5_decoder* dec, const rpx_encoder* enc, const Prefill& p, const __nv_bfloat16* cross_kv,
+                   uint8_t* base, const SeqWs& sw, const int64_t* d_labels, int B, int out_len, float* d_logits,
+                   double* d_seq_logprob, int32_t* d_seq_count, cudaStream_t st) {
+  const rpx_t5_config& c = dec->cfg;
+  const int D = c.d_model, V = c.vocab_size, P = dec->n_parts;
+  const int T_enc = p.T_enc, T_dec = p.T_dec;
+  const Workspace dw = carve(enc, base + sw.dec_off, T_dec > 0 ? T_dec : 1, B);
+  RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, dec->h_cu.data() + B + 1, ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (T_dec > 0) {
+    pack_decoder_kernel<<<ceil_div(T_dec, 256), 256, 0, st>>>(d_labels, dw.cu_tokens, dw.ids, sw.targets, B, out_len,
+                                                              T_dec, dec->start_id);
+    RPX_CUDA_OK(cudaGetLastError());
+    PdlScope pdl_scope(T_dec <= kPdlMaxTokens && T_enc <= kPdlMaxTokens);
+    RPX_TRY(launch_embed(dw.ids, dec->emb, dw.h32, dw.h16, dw.ssA, T_dec, P, T_dec, D, st));
+    float* ss_in = dw.ssA;
+    float* ss_other = dw.ssB;
+    for (int l = 0; l < c.num_layers; ++l)
+      RPX_TRY(decoder_layer(dec, dec->layers[l], l, dw, T_dec, B, p.max_dec, cross_kv, T_enc, p.ew.cu_tokens, &ss_in,
+                            &ss_other, st));
+    // ---- head
+    EpiWsStoreF32Scaled::Params ep{sw.logits, V, RowScale{ss_in, P, T_dec, 1.0f / (float)D, c.ln_eps}};
+    RPX_TRY((launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(dw.h16, D, dec->head, D, T_dec, V, D, ep, st)));
+    token_logprob_kernel<<<ceil_div(T_dec, 8), 256, 0, st>>>(sw.logits, sw.targets, sw.tok_lp, T_dec, V);
+    RPX_CUDA_OK(cudaGetLastError());
+  }
+  seq_logprob_kernel<<<ceil_div(B, 128), 128, 0, st>>>(sw.tok_lp, sw.targets, dw.cu_tokens, d_seq_logprob, d_seq_count,
+                                                       B);
+  RPX_CUDA_OK(cudaGetLastError());
+  if (d_logits) {
+    const int64_t rows = (int64_t)B * out_len;
+    scatter_logits_kernel<<<(unsigned)ceil_div64(rows, 8), 256, 0, st>>>(sw.logits, dw.cu_tokens, d_logits, rows,
+                                                                         out_len, V);
+    RPX_CUDA_OK(cudaGetLastError());
+  }
+  return RPX_OK;
+}
+
+// Stage 3, the search half: beam or greedy search over the prefill's cross K / V, the results into d_sequences /
+// d_scores; then one synchronisation, after which dec->h_poll holds [2] out_len, [3] the encoder's id-range flag,
+// [4] the step at which the last search ended.  init_search must have run.
+int search(rpx_t5_decoder* dec, const rpx_encoder* enc, const Prefill& p, uint8_t* base, const GenWs& g, int B, int nb,
+           int num_return, int ML, double length_penalty, int eos_id, int64_t* d_sequences, float* d_scores,
+           const rpx_generate_trace* trace, cudaStream_t st) {
+  const int R = B * nb, V = dec->cfg.vocab_size;
+  const Workspace dw = carve(enc, base + g.dec_off, R, B);
+  int32_t* cu_beam = dec->h_cu.data() + 2 * B + 2;  // the beams' query offsets, b nb
+  for (int b = 0; b <= B; ++b) cu_beam[b] = b * nb;
+  RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, cu_beam, ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
+  GenerateInitArgs ia{g.tokens, nb > 1 ? g.lin : nullptr, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.state,
+                      g.counters, g.counters + 1, g.counters + 2, R, nb > 1 ? B : R, nb, ML, dec->start_id};
+  RPX_TRY(launch_generate_init(ia, st));
+
+  // ---- the steps, enqueued in blocks; the done-state count of the block before is read while a block runs
+  const int states = nb > 1 ? B : R;
+  int t = 0, blk = 0;
+  {
+    PdlScope pdl_scope(true);
+    while (t <= ML - 2) {
+      const int t_end = t + kPollSteps < ML - 1 ? t + kPollSteps : ML - 1;
+      for (; t < t_end; ++t) {
+        RPX_TRY(decode_step(dec, enc, g, dw, p.ew.cu_tokens, p.T_enc, B, nb, ML, t, st));
+        const bool tr = trace && t < trace->max_steps;
+        BeamStepArgs sa{g.logits, g.tokens, g.lin, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.fin_seq, g.state,
+                        g.counters, g.counters + 2, tr ? trace->d_scores + (size_t)t * R * V : nullptr,
+                        tr ? trace->d_parents + (size_t)t * R : nullptr, tr ? trace->d_tokens + (size_t)t * R : nullptr,
+                        (float)pow((double)(t + 1), length_penalty), t, R, nb, V, ML, eos_id};
+        RPX_TRY(launch_search_step(sa, states, st));
+      }
+      RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + (blk & 1), g.counters, 4, cudaMemcpyDeviceToHost, st));
+      RPX_CUDA_OK(cudaEventRecord(dec->poll_ev[blk & 1], st));
+      if (blk > 0) {
+        RPX_CUDA_OK(cudaEventSynchronize(dec->poll_ev[(blk - 1) & 1]));
+        if (dec->h_poll[(blk - 1) & 1] == states) break;
+      }
+      ++blk;
+    }
+  }
+  GenerateFinishArgs fa{g.tokens, g.fin_score, g.fin_len, g.fin_seq, g.state, d_sequences, d_scores, g.counters + 1, R,
+                        nb, num_return, ML, dec->start_id, nb > 1 && dec->start_id == 0 ? eos_id : dec->start_id};
+  RPX_TRY(launch_generate_finish(fa, nb > 1 ? B : R, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 2, g.counters + 1, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 3, p.ew.flag, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 4, g.counters + 2, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaStreamSynchronize(st));
+  return RPX_OK;
+}
 
 }  // namespace
 }  // namespace rpx
@@ -495,7 +718,7 @@ int rpx_t5_decoder_destroy(rpx_t5_decoder* dec) {
 size_t rpx_seq2seq_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch, int32_t in_len,
                                    int32_t out_len) {
   if (!dec || !enc || batch <= 0 || in_len <= 0 || out_len <= 0 || check_pair(dec, enc) != RPX_OK) return 0;
-  return carve_seq(dec, enc, nullptr, batch, in_len, out_len).total;
+  return carve_prefill(dec, enc, nullptr, batch, in_len).total + carve_seq(dec, enc, nullptr, batch, out_len).total;
 }
 
 int rpx_seq2seq_forward(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
@@ -505,99 +728,27 @@ int rpx_seq2seq_forward(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_
   RPX_REQUIRE(dec && enc && d_input_ids && d_labels && d_seq_logprob && d_seq_count && d_workspace, RPX_ERR_INVALID,
               "rpx_seq2seq_forward: null argument");
   RPX_TRY(check_pair(dec, enc));
-  RPX_REQUIRE(batch > 0 && in_len > 0 && out_len > 0, RPX_ERR_INVALID, "rpx_seq2seq_forward: batch=%d in_len=%d out_len=%d",
-              batch, in_len, out_len);
-  RPX_REQUIRE(batch <= 65535, RPX_ERR_UNSUPPORTED, "rpx_seq2seq_forward: batch=%d exceeds the 65535 grid limit", batch);
-  RPX_REQUIRE((int64_t)batch * in_len < (int64_t)INT32_MAX && (int64_t)batch * out_len < (int64_t)INT32_MAX,
-              RPX_ERR_UNSUPPORTED, "rpx_seq2seq_forward: batch too large");
+  RPX_TRY(check_seq_args("rpx_seq2seq_forward", batch, in_len, out_len, d_logits));
   RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
-  RPX_REQUIRE(d_logits == nullptr || (reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, RPX_ERR_INVALID,
-              "rpx_seq2seq_forward: d_logits must be 16-byte aligned");
-  const rpx_t5_config& c = dec->cfg;
-  const int D = c.d_model, V = c.vocab_size, P = dec->n_parts;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* base = static_cast<uint8_t*>(d_workspace);
-  const SeqWs sw = carve_seq(dec, enc, base, batch, in_len, out_len);
-  RPX_REQUIRE(sw.total <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu", sw.total,
-              workspace_bytes);
-  const Workspace e_max = carve(enc, base + sw.enc_off, (int64_t)batch * in_len, batch);
-  const Workspace d_max = carve(enc, base + sw.dec_off, (int64_t)batch * out_len, batch);
+  const PrefillWs pw = carve_prefill(dec, enc, base, batch, in_len);
+  uint8_t* tail = base + pw.total;
+  const SeqWs sw = carve_seq(dec, enc, tail, batch, out_len);
+  RPX_REQUIRE(pw.total + sw.total <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu",
+              pw.total + sw.total, workspace_bytes);
+  const Workspace d_max = carve(enc, tail + sw.dec_off, (int64_t)batch * out_len, batch);
 
-  // ---- lengths: the state mask's and the labels', read back together
-  RPX_CUDA_OK(cudaMemsetAsync(e_max.flag, 0, 4, st));
-  RPX_CUDA_OK(cudaMemsetAsync(d_max.flag, 0, 4, st));
-  auto& h = dec->h_lens;
-  h.assign(2 * (size_t)batch + 2, in_len);
-  if (d_attention_mask) RPX_TRY(launch_mask_lengths(d_attention_mask, e_max.lens, e_max.flag, batch, in_len, st));
-  label_lengths_kernel<<<ceil_div(batch, 8), 256, 0, st>>>(d_labels, d_max.lens, d_max.flag, batch, out_len, V);
-  RPX_CUDA_OK(cudaGetLastError());
-  if (d_attention_mask) {
-    RPX_CUDA_OK(cudaMemcpyAsync(h.data(), e_max.lens, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
-    RPX_CUDA_OK(cudaMemcpyAsync(&h[batch], e_max.flag, 4, cudaMemcpyDeviceToHost, st));
-  } else {
-    h[batch] = 0;
-  }
-  RPX_CUDA_OK(cudaMemcpyAsync(&h[batch + 1], d_max.lens, (size_t)batch * 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(&h[2 * batch + 1], d_max.flag, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaStreamSynchronize(st));
-  RPX_REQUIRE(h[batch] == 0, RPX_ERR_MASK,
-              "attention_mask must be a right-padded prefix of ones with at least one token per row");
-  RPX_REQUIRE(h[2 * batch + 1] == 0, RPX_ERR_INVALID, "labels must be -100 or ids in [0, %d)", V);
-
-  auto& cu = dec->h_cu;  // [0, B]: encoder offsets, [B + 1, 2B + 1]: decoder offsets
-  cu.assign(2 * (size_t)batch + 2, 0);
-  int max_enc = 0, max_dec = 0;
-  for (int b = 0; b < batch; ++b) {
-    cu[b + 1] = cu[b] + h[b];
-    cu[batch + 2 + b] = cu[batch + 1 + b] + h[batch + 1 + b];
-    max_enc = h[b] > max_enc ? h[b] : max_enc;
-    max_dec = h[batch + 1 + b] > max_dec ? h[batch + 1 + b] : max_dec;
-  }
-  const int T_enc = cu[batch], T_dec = cu[2 * batch + 1];
-  const Workspace ew = carve(enc, base + sw.enc_off, T_enc, batch);
-  const Workspace dw = carve(enc, base + sw.dec_off, T_dec > 0 ? T_dec : 1, batch);
-  RPX_CUDA_OK(cudaMemcpyAsync(ew.cu_tokens, cu.data(), ((size_t)batch + 1) * 4, cudaMemcpyHostToDevice, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, cu.data() + batch + 1, ((size_t)batch + 1) * 4, cudaMemcpyHostToDevice, st));
-  RPX_TRY(launch_pack_ids(d_input_ids, ew.cu_tokens, ew.ids, batch, in_len, T_enc, V, ew.flag, st));
-  if (T_dec > 0) {
-    pack_decoder_kernel<<<ceil_div(T_dec, 256), 256, 0, st>>>(d_labels, dw.cu_tokens, dw.ids, sw.targets, batch, out_len,
-                                                              T_dec, dec->start_id);
-    RPX_CUDA_OK(cudaGetLastError());
-  }
-
-  // ---- encoder, cross K / V of every decoder layer
-  RPX_TRY(forward(enc, ew, T_enc, batch, max_enc, OutKind::kResidual, 0, nullptr, 0, st));
-  if (T_dec > 0) {
-    PdlScope pdl_scope(T_dec <= kPdlMaxTokens && T_enc <= kPdlMaxTokens);
-    RPX_TRY(qkv_gemm(false, T_enc, ew.h16, dec->cross_kv, dec->n_kv, D,
-                     RowScale{ew.ssA, enc->n_parts, T_enc, 1.0f / (float)D, c.ln_eps}, sw.cross_kv, nullptr, 0, st));
-    // ---- decoder
-    RPX_TRY(launch_embed(dw.ids, dec->emb, dw.h32, dw.h16, dw.ssA, T_dec, P, T_dec, D, st));
-    float* ss_in = dw.ssA;
-    float* ss_other = dw.ssB;
-    for (int l = 0; l < c.num_layers; ++l)
-      RPX_TRY(decoder_layer(dec, dec->layers[l], l, dw, T_dec, batch, max_dec, sw.cross_kv, T_enc, ew.cu_tokens, &ss_in,
-                            &ss_other, st));
-    // ---- head
-    EpiWsStoreF32Scaled::Params ep{sw.logits, V, RowScale{ss_in, P, T_dec, 1.0f / (float)D, c.ln_eps}};
-    RPX_TRY((launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(dw.h16, D, dec->head, D, T_dec, V, D, ep, st)));
-    token_logprob_kernel<<<ceil_div(T_dec, 8), 256, 0, st>>>(sw.logits, sw.targets, sw.tok_lp, T_dec, V);
-    RPX_CUDA_OK(cudaGetLastError());
-  }
-  seq_logprob_kernel<<<ceil_div(batch, 128), 128, 0, st>>>(sw.tok_lp, sw.targets, dw.cu_tokens, d_seq_logprob, d_seq_count,
-                                                           batch);
-  RPX_CUDA_OK(cudaGetLastError());
-  if (d_logits) {
-    const int64_t rows = (int64_t)batch * out_len;
-    scatter_logits_kernel<<<(unsigned)ceil_div64(rows, 8), 256, 0, st>>>(sw.logits, dw.cu_tokens, d_logits, rows,
-                                                                         out_len, V);
-    RPX_CUDA_OK(cudaGetLastError());
-  }
+  Prefill p;
+  RPX_TRY(prefill(dec, enc, d_input_ids, d_attention_mask, batch, in_len, d_labels, out_len, d_max.lens, d_max.flag,
+                  base, pw, false, &p, st));
+  RPX_TRY(teacher_forced(dec, enc, p, pw.cross_kv, tail, sw, d_labels, batch, out_len, d_logits, d_seq_logprob,
+                         d_seq_count, st));
   // ids outside [0, vocab) are reported after the fact (the forward ran with id 0 in their place)
   int32_t flag = 0;
-  RPX_CUDA_OK(cudaMemcpyAsync(&flag, ew.flag, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(&flag, p.ew.flag, 4, cudaMemcpyDeviceToHost, st));
   RPX_CUDA_OK(cudaStreamSynchronize(st));
-  RPX_REQUIRE((flag & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", V);
+  RPX_REQUIRE((flag & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", dec->cfg.vocab_size);
   return RPX_OK;
 }
 
@@ -606,7 +757,8 @@ size_t rpx_seq2seq_generate_workspace_bytes(const rpx_t5_decoder* dec, const rpx
   if (!dec || !enc || batch <= 0 || in_len <= 0 || num_beams <= 0 || num_beams > kMaxBeams || max_length < 2 ||
       check_pair(dec, enc) != RPX_OK)
     return 0;
-  return carve_gen(dec, enc, nullptr, batch, in_len, num_beams, max_length).total;
+  return carve_prefill(dec, enc, nullptr, batch, in_len).total +
+         carve_gen(dec, enc, nullptr, nullptr, batch, num_beams, max_length).total;
 }
 
 int rpx_seq2seq_generate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
@@ -617,114 +769,79 @@ int rpx_seq2seq_generate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d
   RPX_REQUIRE(dec && enc && d_input_ids && d_sequences && h_out_len && d_workspace, RPX_ERR_INVALID,
               "rpx_seq2seq_generate: null argument");
   RPX_TRY(check_pair(dec, enc));
-  const rpx_t5_config& c = dec->cfg;
-  const int V = c.vocab_size;
-  RPX_REQUIRE(batch > 0 && in_len > 0, RPX_ERR_INVALID, "rpx_seq2seq_generate: batch=%d in_len=%d", batch, in_len);
-  RPX_REQUIRE(num_beams >= 1 && num_beams <= kMaxBeams, RPX_ERR_INVALID,
-              "rpx_seq2seq_generate: num_beams=%d outside [1, %d]", num_beams, kMaxBeams);
-  RPX_REQUIRE(num_return >= 1 && num_return <= num_beams, RPX_ERR_INVALID,
-              "rpx_seq2seq_generate: num_return=%d outside [1, num_beams=%d]", num_return, num_beams);
-  RPX_REQUIRE(num_beams == 1 || 2 * num_beams <= V, RPX_ERR_INVALID,
-              "rpx_seq2seq_generate: 2 * num_beams=%d exceeds vocab_size=%d", 2 * num_beams, V);
-  RPX_REQUIRE(num_beams == 1 || d_scores, RPX_ERR_INVALID, "rpx_seq2seq_generate: beam search needs d_scores");
-  RPX_REQUIRE(max_length >= 2, RPX_ERR_INVALID, "rpx_seq2seq_generate: max_length=%d must be at least 2", max_length);
-  RPX_REQUIRE(eos_id >= 0 && eos_id < V, RPX_ERR_INVALID, "rpx_seq2seq_generate: eos_id=%d outside [0, %d)", eos_id, V);
-  RPX_REQUIRE(num_beams == 1 || beam_step_smem_bytes(num_beams, V) <= kMaxStepSmem, RPX_ERR_UNSUPPORTED,
-              "rpx_seq2seq_generate: num_beams * vocab_size=%d candidates exceed one CTA's shared memory",
-              num_beams * V);
-  RPX_REQUIRE(batch <= 65535 && (int64_t)batch * in_len < (int64_t)INT32_MAX &&
-                  (int64_t)batch * num_beams * max_length < (int64_t)INT32_MAX,
-              RPX_ERR_UNSUPPORTED, "rpx_seq2seq_generate: batch too large");
+  RPX_TRY(check_gen_args("rpx_seq2seq_generate", batch, in_len, num_beams, num_return, max_length, eos_id, d_scores,
+                         dec->cfg.vocab_size));
   RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
   RPX_REQUIRE(!trace || (trace->d_scores && trace->d_parents && trace->d_tokens && trace->max_steps >= 0),
               RPX_ERR_INVALID, "rpx_seq2seq_generate: incomplete trace");
-  const int B = batch, nb = num_beams, R = B * nb, ML = max_length, D = c.d_model;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* base = static_cast<uint8_t*>(d_workspace);
-  const GenWs g = carve_gen(dec, enc, base, B, in_len, nb, ML);
-  RPX_REQUIRE(g.total <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu", g.total,
-              workspace_bytes);
-  if (!dec->h_poll) {
-    RPX_TRY(configure_search_step(kMaxStepSmem));
-    RPX_CUDA_OK(cudaHostAlloc(reinterpret_cast<void**>(&dec->h_poll), 32, cudaHostAllocDefault));
-    for (cudaEvent_t& ev : dec->poll_ev) RPX_CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-  }
-  const Workspace e_max = carve(enc, base + g.enc_off, (int64_t)B * in_len, B);
+  const PrefillWs pw = carve_prefill(dec, enc, base, batch, in_len);
+  uint8_t* tail = base + pw.total;
+  const GenWs g = carve_gen(dec, enc, tail, pw.cross_kv, batch, num_beams, max_length);
+  RPX_REQUIRE(pw.total + g.total <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu",
+              pw.total + g.total, workspace_bytes);
+  RPX_TRY(init_search(dec));
 
-  // ---- the states' lengths
-  RPX_CUDA_OK(cudaMemsetAsync(e_max.flag, 0, 4, st));
-  auto& h = dec->h_lens;
-  h.assign((size_t)B + 1, in_len);
-  h[B] = 0;
-  if (d_attention_mask) {
-    RPX_TRY(launch_mask_lengths(d_attention_mask, e_max.lens, e_max.flag, B, in_len, st));
-    RPX_CUDA_OK(cudaMemcpyAsync(h.data(), e_max.lens, (size_t)B * 4, cudaMemcpyDeviceToHost, st));
-    RPX_CUDA_OK(cudaMemcpyAsync(&h[B], e_max.flag, 4, cudaMemcpyDeviceToHost, st));
-    RPX_CUDA_OK(cudaStreamSynchronize(st));
-    RPX_REQUIRE(h[B] == 0, RPX_ERR_MASK,
-                "attention_mask must be a right-padded prefix of ones with at least one token per row");
-  }
-  auto& cu = dec->h_cu;  // [0, B]: encoder offsets, [B + 1, 2B + 1]: the beams' query offsets (b nb)
-  cu.assign(2 * (size_t)B + 2, 0);
-  int max_enc = 0;
-  for (int b = 0; b < B; ++b) {
-    cu[b + 1] = cu[b] + h[b];
-    cu[B + 2 + b] = (b + 1) * nb;
-    max_enc = h[b] > max_enc ? h[b] : max_enc;
-  }
-  const int T_enc = cu[B];
-  const Workspace ew = carve(enc, base + g.enc_off, T_enc, B);
-  const Workspace dw = carve(enc, base + g.dec_off, R, B);
-  RPX_CUDA_OK(cudaMemcpyAsync(ew.cu_tokens, cu.data(), ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, cu.data() + B + 1, ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
-  RPX_TRY(launch_pack_ids(d_input_ids, ew.cu_tokens, ew.ids, B, in_len, T_enc, V, ew.flag, st));
-  // the host vectors stay untouched until the next call, which synchronises before reusing them
-  GenerateInitArgs ia{g.tokens, nb > 1 ? g.lin : nullptr, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.state,
-                      g.counters, g.counters + 1, g.counters + 2, R, nb > 1 ? B : R, nb, ML, dec->start_id};
-  RPX_TRY(launch_generate_init(ia, st));
-
-  // ---- prefill: encoder, then the cross K / V of every decoder layer, once per state
-  RPX_TRY(forward(enc, ew, T_enc, B, max_enc, OutKind::kResidual, 0, nullptr, 0, st));
-  {
-    PdlScope pdl_scope(T_enc <= kPdlMaxTokens);
-    RPX_TRY(qkv_gemm(false, T_enc, ew.h16, dec->cross_kv, dec->n_kv, D,
-                     RowScale{ew.ssA, enc->n_parts, T_enc, 1.0f / (float)D, c.ln_eps}, g.cross_kv, nullptr, 0, st));
-  }
-
-  // ---- the steps, enqueued in blocks; the done-state count of the block before is read while a block runs
-  const int states = nb > 1 ? B : R;
-  int t = 0, blk = 0;
-  {
-    PdlScope pdl_scope(true);
-    while (t <= ML - 2) {
-      const int t_end = t + kPollSteps < ML - 1 ? t + kPollSteps : ML - 1;
-      for (; t < t_end; ++t) {
-        RPX_TRY(decode_step(dec, enc, g, dw, ew.cu_tokens, T_enc, B, nb, ML, t, st));
-        const bool tr = trace && t < trace->max_steps;
-        BeamStepArgs sa{g.logits, g.tokens, g.lin, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.fin_seq, g.state,
-                        g.counters, g.counters + 2, tr ? trace->d_scores + (size_t)t * R * V : nullptr,
-                        tr ? trace->d_parents + (size_t)t * R : nullptr, tr ? trace->d_tokens + (size_t)t * R : nullptr,
-                        (float)pow((double)(t + 1), length_penalty), t, R, nb, V, ML, eos_id};
-        RPX_TRY(launch_search_step(sa, states, st));
-      }
-      RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + (blk & 1), g.counters, 4, cudaMemcpyDeviceToHost, st));
-      RPX_CUDA_OK(cudaEventRecord(dec->poll_ev[blk & 1], st));
-      if (blk > 0) {
-        RPX_CUDA_OK(cudaEventSynchronize(dec->poll_ev[(blk - 1) & 1]));
-        if (dec->h_poll[(blk - 1) & 1] == states) break;
-      }
-      ++blk;
-    }
-  }
-  GenerateFinishArgs fa{g.tokens, g.fin_score, g.fin_len, g.fin_seq, g.state, d_sequences, d_scores, g.counters + 1, R,
-                        nb, num_return, ML, dec->start_id, nb > 1 && dec->start_id == 0 ? eos_id : dec->start_id};
-  RPX_TRY(launch_generate_finish(fa, nb > 1 ? B : R, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 2, g.counters + 1, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 3, ew.flag, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 4, g.counters + 2, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaStreamSynchronize(st));
+  Prefill p;
+  RPX_TRY(prefill(dec, enc, d_input_ids, d_attention_mask, batch, in_len, nullptr, 0, nullptr, nullptr, base, pw, true,
+                  &p, st));
+  RPX_TRY(search(dec, enc, p, tail, g, batch, num_beams, num_return, max_length, length_penalty, eos_id, d_sequences,
+                 d_scores, trace, st));
   // ids outside [0, vocab) are reported after the fact (the search ran with id 0 in their place)
-  RPX_REQUIRE((dec->h_poll[3] & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", V);
+  RPX_REQUIRE((dec->h_poll[3] & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", dec->cfg.vocab_size);
+  *h_out_len = dec->h_poll[2];
+  if (h_steps) *h_steps = dec->h_poll[4];
+  return RPX_OK;
+}
+
+size_t rpx_seq2seq_evaluate_workspace_bytes(const rpx_t5_decoder* dec, const rpx_encoder* enc, int32_t batch,
+                                            int32_t in_len, int32_t out_len, int32_t num_beams, int32_t max_length) {
+  if (!dec || !enc || batch <= 0 || in_len <= 0 || out_len <= 0 || num_beams <= 0 || num_beams > kMaxBeams ||
+      max_length < 2 || check_pair(dec, enc) != RPX_OK)
+    return 0;
+  const size_t seq = carve_seq(dec, enc, nullptr, batch, out_len).total;
+  const size_t gen = carve_gen(dec, enc, nullptr, nullptr, batch, num_beams, max_length).total;
+  return carve_prefill(dec, enc, nullptr, batch, in_len).total + (seq > gen ? seq : gen);
+}
+
+int rpx_seq2seq_evaluate(rpx_t5_decoder* dec, rpx_encoder* enc, const int64_t* d_input_ids,
+                         const int64_t* d_attention_mask, int32_t batch, int32_t in_len, const int64_t* d_labels,
+                         int32_t out_len, float* d_logits, double* d_seq_logprob, int32_t* d_seq_count,
+                         int32_t num_beams, int32_t num_return, int32_t max_length, double length_penalty,
+                         int32_t eos_id, int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                         void* d_workspace, size_t workspace_bytes, void* stream) {
+  RPX_REQUIRE(dec && enc && d_input_ids && d_labels && d_seq_logprob && d_seq_count && d_sequences && h_out_len &&
+                  d_workspace,
+              RPX_ERR_INVALID, "rpx_seq2seq_evaluate: null argument");
+  RPX_TRY(check_pair(dec, enc));
+  RPX_TRY(check_seq_args("rpx_seq2seq_evaluate", batch, in_len, out_len, d_logits));
+  RPX_TRY(check_gen_args("rpx_seq2seq_evaluate", batch, in_len, num_beams, num_return, max_length, eos_id, d_scores,
+                         dec->cfg.vocab_size));
+  RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* base = static_cast<uint8_t*>(d_workspace);
+  const PrefillWs pw = carve_prefill(dec, enc, base, batch, in_len);
+  // the two halves share the regions after the prefill's: the search starts after the teacher-forced half's last
+  // kernel on the same stream, and reads nothing of it
+  uint8_t* tail = base + pw.total;
+  const SeqWs sw = carve_seq(dec, enc, tail, batch, out_len);
+  const GenWs g = carve_gen(dec, enc, tail, pw.cross_kv, batch, num_beams, max_length);
+  const size_t need = pw.total + (sw.total > g.total ? sw.total : g.total);
+  RPX_REQUIRE(need <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu", need,
+              workspace_bytes);
+  const Workspace d_max = carve(enc, tail + sw.dec_off, (int64_t)batch * out_len, batch);
+  RPX_TRY(init_search(dec));
+
+  Prefill p;
+  RPX_TRY(prefill(dec, enc, d_input_ids, d_attention_mask, batch, in_len, d_labels, out_len, d_max.lens, d_max.flag,
+                  base, pw, true, &p, st));
+  RPX_TRY(teacher_forced(dec, enc, p, pw.cross_kv, tail, sw, d_labels, batch, out_len, d_logits, d_seq_logprob,
+                         d_seq_count, st));
+  RPX_TRY(search(dec, enc, p, tail, g, batch, num_beams, num_return, max_length, length_penalty, eos_id, d_sequences,
+                 d_scores, nullptr, st));
+  // ids outside [0, vocab) are reported once, after both halves ran with id 0 in their place
+  RPX_REQUIRE((dec->h_poll[3] & 2) == 0, RPX_ERR_INVALID, "input_ids contains ids outside [0, %d)", dec->cfg.vocab_size);
   *h_out_len = dec->h_poll[2];
   if (h_steps) *h_steps = dec->h_poll[4];
   return RPX_OK;

@@ -77,6 +77,30 @@ def load_hf_checkpoint(path: str) -> Tuple[Dict, Dict[str, torch.Tensor]]:
     return cfg, {k: v.float() for k, v in sd.items()}
 
 
+# Keys HF ties to `shared.weight` and does not save beside it.
+_TIED_KEYS = ("encoder.embed_tokens.weight", "decoder.embed_tokens.weight")
+
+
+def save_hf_dir(save_directory: str, config: Dict, state_dict: Dict[str, torch.Tensor], architecture: str) -> None:
+    """Writes an HF checkpoint directory as `save_pretrained` lays it out: `config.json` (with `architectures`
+    defaulting to `[architecture]` and `model_type` to "t5") and fp32 `model.safetensors`.  The embedding copies HF
+    ties to `shared.weight` are left out, and so is a tied `lm_head.weight` (`tie_word_embeddings` absent or
+    true)."""
+    from safetensors.torch import save_file
+
+    os.makedirs(save_directory, exist_ok=True)
+    cfg = dict(config)
+    cfg.setdefault("architectures", [architecture])
+    cfg.setdefault("model_type", "t5")
+    with open(os.path.join(save_directory, "config.json"), "w") as fh:
+        json.dump(cfg, fh, indent=1)
+    tied = set(_TIED_KEYS) if "shared.weight" in state_dict else set()
+    if cfg.get("tie_word_embeddings", True) is not False and "shared.weight" in state_dict:
+        tied.add("lm_head.weight")
+    tensors = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in state_dict.items() if k not in tied}
+    save_file(tensors, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
+
+
 def required_weight_keys(config: Dict) -> List[str]:
     """Every state-dict key the encoder engine reads (HF T5EncoderModel names)."""
     keys = [_REL_BIAS_KEY, "encoder.final_layer_norm.weight"]
@@ -194,18 +218,7 @@ class T5EncoderEngine:
         saves the retriever's encoder next to the generator): writes `config.json` and
         `model.safetensors` with the fp32 weights this engine was built from, loadable by
         `AutoModelForTextEncoding.from_pretrained(dir)` and by `load_hf`."""
-        from safetensors.torch import save_file
-
-        os.makedirs(save_directory, exist_ok=True)
-        cfg = dict(self.config)
-        cfg.setdefault("architectures", ["T5EncoderModel"])
-        cfg.setdefault("model_type", "t5")
-        with open(os.path.join(save_directory, "config.json"), "w") as fh:
-            json.dump(cfg, fh, indent=1)
-        sd = self._state_dict
-        tensors = {k: v.detach().to("cpu", torch.float32).contiguous() for k, v in sd.items()
-                   if k != "encoder.embed_tokens.weight" or "shared.weight" not in sd}
-        save_file(tensors, os.path.join(save_directory, "model.safetensors"), metadata={"format": "pt"})
+        save_hf_dir(save_directory, self.config, self._state_dict, "T5EncoderModel")
 
     @classmethod
     def from_hf_dir(cls, path: str, device, **kw) -> "T5EncoderEngine":

@@ -211,7 +211,8 @@ class Seq2SeqOutput(NamedTuple):
 
 
 class T5GeneratorEngine:
-    """ByT5/T5 encoder-decoder, teacher-forced, on one GPU (`rpx_seq2seq_forward`)."""
+    """ByT5/T5 encoder-decoder on one GPU: the teacher-forced forward (`rpx_seq2seq_forward`), `generate`
+    (`rpx_seq2seq_generate`), and both on one encoder pass (`evaluate`, `rpx_seq2seq_evaluate`)."""
 
     def __init__(self, config: Dict, state_dict: Dict[str, torch.Tensor], device: Union[int, str, torch.device],
                  generation_config: Optional[Dict] = None) -> None:
@@ -228,6 +229,8 @@ class T5GeneratorEngine:
         self.encoder = T5EncoderEngine(config, state_dict, self.device)
         self._handle = C.c_void_p()
         self._ws: Optional[torch.Tensor] = None
+        self.hparams: Dict[str, Any] = {}
+        self.last_steps = 0  # decoder steps of the last `evaluate`'s search (HF's count)
         with torch.cuda.device(self.device):
             cfg = _native.T5Config(
                 vocab_size=config["vocab_size"], d_model=config["d_model"], d_kv=config["d_kv"], d_ff=config["d_ff"],
@@ -272,6 +275,22 @@ class T5GeneratorEngine:
             with open(gc_path) as fh:
                 kw["generation_config"] = json.load(fh)
         return cls(cfg, sd, device, **kw)
+
+    @classmethod
+    def load(cls, ckpt_path: str, device, freeze: bool = True, config: Optional[Dict] = None) -> "T5GeneratorEngine":
+        """The reference's `RetrievalAugmentedGenerator.load` (generation/model.py, common.py:load_checkpoint): a
+        Lightning `.ckpt` written by the reference's training, or a DeepSpeed ZeRO checkpoint directory.  The model
+        config is `config`, else `model_name`'s cached config, else the one the weights' shapes give
+        (`checkpoint.load_generator_checkpoint`); `generation_config.json` is `model_name`'s cached one when there
+        is one.  `engine.hparams` holds the checkpoint's hyper-parameters.  `freeze` is accepted for parity: the
+        engine keeps no gradients."""
+        from .checkpoint import cached_config, load_generator_checkpoint
+
+        cfg, sd, hp = load_generator_checkpoint(ckpt_path, config)
+        gen_cfg = cached_config(hp["model_name"], "generation_config.json") if hp.get("model_name") else None
+        engine = cls(cfg, sd, device, generation_config=gen_cfg)
+        engine.hparams = hp
+        return engine
 
     def close(self) -> None:
         if getattr(self, "_handle", None) and self._handle.value:
@@ -321,32 +340,48 @@ class T5GeneratorEngine:
         if asked:
             raise NotImplementedError(f"T5GeneratorEngine runs the teacher-forced forward from labels only; "
                                       f"not supported: {asked}")
-        if input_ids is None or input_ids.dim() != 2:
-            raise ValueError("input_ids must be a [batch, seq_len] tensor")
-        if labels is None or labels.dim() != 2 or labels.shape[0] != input_ids.shape[0]:
-            raise ValueError("labels must be a [batch, tgt_len] tensor with input_ids' batch")
-        ids = input_ids.to(device=self.device, dtype=torch.int64).contiguous()
-        mask = None
-        if attention_mask is not None:
-            if attention_mask.shape != input_ids.shape:
-                raise ValueError(f"attention_mask {tuple(attention_mask.shape)} != input_ids {tuple(input_ids.shape)}")
-            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
-        lab = labels.to(device=self.device, dtype=torch.int64).contiguous()
+        ids, mask = self._states(input_ids, attention_mask)
+        lab = self._labels(labels, ids.shape[0])
         B, L_in = ids.shape
         L_out = lab.shape[1]
-        logits = torch.empty(B, L_out, self.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
-        seq_lp = torch.empty(B, dtype=torch.float64, device=self.device)
-        seq_n = torch.empty(B, dtype=torch.int32, device=self.device)
+        logits, seq_lp, seq_n = self._loss_outputs(B, L_out, return_logits)
         with torch.cuda.device(self.device):
             ws = self._workspace(B, L_in, L_out)
             _native.check(self.lib.rpx_seq2seq_forward(
                 self._handle, self.encoder._handle, ids.data_ptr(), None if mask is None else mask.data_ptr(), B, L_in,
                 lab.data_ptr(), L_out, None if logits is None else logits.data_ptr(), seq_lp.data_ptr(),
                 seq_n.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(self.device)))
-        loss = -seq_lp.sum() / seq_n.sum().double()  # 0 / 0 = NaN when nothing counts, as HF's empty mean
-        return Seq2SeqOutput(loss, logits, seq_lp, seq_n)
+        return self._seq2seq_output(logits, seq_lp, seq_n)
 
     forward = __call__
+
+    def _states(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor]):
+        """Device int64 ids and mask (or None) of a [batch, seq_len] batch of states."""
+        if input_ids is None or input_ids.dim() != 2:
+            raise ValueError("input_ids must be a [batch, seq_len] tensor")
+        ids = input_ids.to(device=self.device, dtype=torch.int64).contiguous()
+        mask = None
+        if attention_mask is not None:
+            if attention_mask.shape != input_ids.shape:
+                raise ValueError(f"attention_mask {tuple(attention_mask.shape)} != input_ids {tuple(input_ids.shape)}")
+            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
+        return ids, mask
+
+    def _labels(self, labels: torch.Tensor, batch: int) -> torch.Tensor:
+        if labels is None or labels.dim() != 2 or labels.shape[0] != batch:
+            raise ValueError("labels must be a [batch, tgt_len] tensor with input_ids' batch")
+        return labels.to(device=self.device, dtype=torch.int64).contiguous()
+
+    def _loss_outputs(self, B: int, L_out: int, return_logits: bool):
+        logits = torch.empty(B, L_out, self.vocab_size, dtype=torch.float32, device=self.device) if return_logits else None
+        seq_lp = torch.empty(B, dtype=torch.float64, device=self.device)
+        seq_n = torch.empty(B, dtype=torch.int32, device=self.device)
+        return logits, seq_lp, seq_n
+
+    @staticmethod
+    def _seq2seq_output(logits, seq_lp: torch.Tensor, seq_n: torch.Tensor) -> Seq2SeqOutput:
+        loss = -seq_lp.sum() / seq_n.sum().double()  # 0 / 0 = NaN when nothing counts, as HF's empty mean
+        return Seq2SeqOutput(loss, logits, seq_lp, seq_n)
 
     def to(self, device=None, *args: Any, **kwargs: Any) -> "T5GeneratorEngine":
         """HF's `model.to(device)`, as the reference calls it after loading a generator: the engine is bound to the
@@ -376,32 +411,68 @@ class T5GeneratorEngine:
         `output_fill_value` does for T5).  `_trace_steps` (tests) records each of the first that many steps and returns
         `(output, trace)`: "scores" [steps, R, V] (log-probs; logits for greedy), "parents" and "tokens" [steps, R],
         and "steps", the decoder steps HF runs for this call (the step at which the last search ended)."""
-        s = generation_settings(self.config, self.generation_config, max_length=max_length, num_beams=num_beams,
-                                do_sample=do_sample, num_return_sequences=num_return_sequences,
-                                length_penalty=length_penalty, early_stopping=early_stopping,
-                                output_scores=output_scores, return_dict_in_generate=return_dict_in_generate,
-                                **unsupported)
+        s = self._generation_settings(max_length=max_length, num_beams=num_beams, do_sample=do_sample,
+                                      num_return_sequences=num_return_sequences, length_penalty=length_penalty,
+                                      early_stopping=early_stopping, output_scores=output_scores,
+                                      return_dict_in_generate=return_dict_in_generate, **unsupported)
+        ids, mask = self._states(input_ids, attention_mask)
+        seqs, scores, trace = self._search(ids, mask, s, int(_trace_steps))
+        if not s.return_dict_in_generate:
+            if trace is not None:
+                return GenerateOutput(seqs, scores), trace
+            return seqs
+        out = self._generate_output(s, seqs, scores)
+        return (out, trace) if trace is not None else out
+
+    def _generation_settings(self, **kwargs: Any) -> GenerationSettings:
+        """`generation_settings` for this engine, and the refusals of ids the engine does not run."""
+        s = generation_settings(self.config, self.generation_config, **kwargs)
         if s.decoder_start_token_id != self.gen_config.start_token_id:
             raise NotImplementedError(f"decoder_start_token_id={s.decoder_start_token_id}: the engine starts every "
                                       f"hypothesis with the config's {self.gen_config.start_token_id}")
         if s.pad_token_id != self.gen_config.start_token_id:
             raise NotImplementedError(f"pad_token_id={s.pad_token_id}: the engine pads with the decoder start id "
                                       f"{self.gen_config.start_token_id}, as `_shift_right` does")
-        if input_ids is None or input_ids.dim() != 2:
-            raise ValueError("input_ids must be a [batch, seq_len] tensor")
-        ids = input_ids.to(device=self.device, dtype=torch.int64).contiguous()
-        mask = None
-        if attention_mask is not None:
-            if attention_mask.shape != input_ids.shape:
-                raise ValueError(f"attention_mask {tuple(attention_mask.shape)} != input_ids {tuple(input_ids.shape)}")
-            mask = attention_mask.to(device=self.device, dtype=torch.int64).contiguous()
-        seqs, scores, trace = self._search(ids, mask, s, int(_trace_steps))
+        return s
+
+    @staticmethod
+    def _generate_output(s: GenerationSettings, seqs: torch.Tensor, scores: Optional[torch.Tensor]):
         if not s.return_dict_in_generate:
-            if trace is not None:
-                return GenerateOutput(seqs, scores), trace
             return seqs
-        out = GenerateOutput(seqs, scores if s.output_scores else None)
-        return (out, trace) if trace is not None else out
+        return GenerateOutput(seqs, scores if s.output_scores else None)
+
+    def evaluate(self, input_ids: torch.Tensor, attention_mask: Optional[torch.Tensor], labels: torch.Tensor, *,
+                 return_logits: bool = False, **generate_kwargs: Any):
+        """`self(input_ids, attention_mask, labels)` and `self.generate(input_ids, attention_mask, **generate_kwargs)`
+        in one call, as the reference's `validation_step` runs them on one batch, with the encoder and the
+        cross-attention K / V computed once for both (`rpx_seq2seq_evaluate`).  Returns `(Seq2SeqOutput, generate
+        output)`, each equal bit for bit to what the two calls return; the settings and refusals are `generate`'s."""
+        s = self._generation_settings(**generate_kwargs)
+        ids, mask = self._states(input_ids, attention_mask)
+        lab = self._labels(labels, ids.shape[0])
+        B, L_in = ids.shape
+        L_out = lab.shape[1]
+        nb, n_ret, ML = s.num_beams, s.num_return_sequences, s.max_length
+        logits, seq_lp, seq_n = self._loss_outputs(B, L_out, return_logits)
+        seqs = torch.empty(B * n_ret, ML, dtype=torch.int64, device=self.device)
+        scores = torch.empty(B * n_ret, dtype=torch.float32, device=self.device) if nb > 1 else None
+        out_len, steps = C.c_int32(0), C.c_int32(0)
+        with torch.cuda.device(self.device):
+            need = self.lib.rpx_seq2seq_evaluate_workspace_bytes(self._handle, self.encoder._handle, B, L_in, L_out, nb,
+                                                                 ML)
+            if need == 0:
+                raise _native.RpxError(_native.RPX_ERR_INVALID, f"no evaluate workspace for batch={B} {L_in}x{L_out} "
+                                       f"num_beams={nb} max_length={ML}")
+            ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            _native.check(self.lib.rpx_seq2seq_evaluate(
+                self._handle, self.encoder._handle, ids.data_ptr(), None if mask is None else mask.data_ptr(), B, L_in,
+                lab.data_ptr(), L_out, None if logits is None else logits.data_ptr(), seq_lp.data_ptr(),
+                seq_n.data_ptr(), nb, n_ret, ML, s.length_penalty, s.eos_token_id, seqs.data_ptr(),
+                None if scores is None else scores.data_ptr(), C.byref(out_len), C.byref(steps), ws.data_ptr(),
+                ws.numel(), _stream_ptr(self.device)))
+        self.last_steps = steps.value
+        return (self._seq2seq_output(logits, seq_lp, seq_n),
+                self._generate_output(s, seqs[:, :out_len.value].contiguous(), scores))
 
     def _search(self, ids: torch.Tensor, mask: Optional[torch.Tensor], s: GenerationSettings, trace_steps: int):
         """rpx_seq2seq_generate on device ids / mask: (sequences [B * n_ret, L_out], scores or None, trace or None)."""

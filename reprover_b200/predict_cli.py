@@ -24,59 +24,21 @@ import os
 import pickle
 from typing import Any, Dict, List, Optional, Tuple
 
+from .cli_args import parse_cli
+
 logger = logging.getLogger("reprover_b200.predict")
 
 USED_KEYS = ("model.num_retrieved", "data.data_path", "data.corpus_path", "data.max_seq_len", "data.eval_batch_size")
 SPLITS = {"predict": ("train", "val", "test"), "validate": ("val",)}
 
 
-def _flatten(tree: Dict[str, Any], prefix: str = "") -> Dict[str, Any]:
-    """{"data": {"max_seq_len": 1024}} -> {"data.max_seq_len": 1024}."""
-    out: Dict[str, Any] = {}
-    for key, value in tree.items():
-        if isinstance(value, dict):
-            out.update(_flatten(value, f"{prefix}{key}."))
-        else:
-            out[f"{prefix}{key}"] = value
-    return out
-
-
 def parse_args(argv: Optional[List[str]] = None) -> Tuple[argparse.Namespace, Dict[str, Any], List[str]]:
-    """(fixed flags, settings by dotted key, ignored keys).  Settings are the config files' in order, then the
-    dotted command-line overrides; override values are read as YAML scalars, as LightningCLI reads them."""
-    import yaml
-
+    """(fixed flags, settings by dotted key, ignored keys), as `cli_args.parse_cli` reads them."""
     parser = argparse.ArgumentParser(description="Dense premise retrieval (predict / validate) on the H100 engine.")
-    parser.add_argument("subcommand", choices=sorted(SPLITS))
-    parser.add_argument("--config", action="append", default=[], help="LightningCLI YAML config (repeatable)")
-    parser.add_argument("--ckpt_path", type=str, default=None, help="Lightning .ckpt file or DeepSpeed ZeRO directory")
-    parser.add_argument("--hf-ckpt", type=str, default=None, help="HF checkpoint directory or hub id")
     parser.add_argument("--output-path", type=str, default="predictions.pickle")
     parser.add_argument("--native-layout", action="store_true",
                         help="pickle this package's own classes instead of the reference's layout")
-    args, rest = parser.parse_known_args(argv)
-    if (args.ckpt_path is None) == (args.hf_ckpt is None):
-        parser.error("pass exactly one of --ckpt_path and --hf-ckpt")
-    settings: Dict[str, Any] = {}
-    for path in args.config:
-        with open(path) as fh:
-            settings.update(_flatten(yaml.safe_load(fh) or {}))
-    i = 0
-    while i < len(rest):
-        tok = rest[i]
-        if not tok.startswith("--"):
-            parser.error(f"unexpected argument {tok!r}")
-        if "=" in tok:
-            key, value = tok[2:].split("=", 1)
-            i += 1
-        else:
-            if i + 1 >= len(rest):
-                parser.error(f"{tok} needs a value")
-            key, value = tok[2:], rest[i + 1]
-            i += 2
-        settings[key] = yaml.safe_load(value)
-    ignored = sorted({k for k in settings if k not in USED_KEYS})
-    return args, settings, ignored
+    return parse_cli(parser, SPLITS, USED_KEYS, argv)
 
 
 def _load_retriever(args: argparse.Namespace, settings: Dict[str, Any]):

@@ -100,3 +100,11 @@ def pad_batch(id_lists: Sequence[Sequence[int]]):
         ids[r, : len(x)] = x
         mask[r, : len(x)] = 1
     return ids, mask
+
+
+def decode(ids: Sequence[int]) -> str:
+    """HF `ByT5Tokenizer.batch_decode(..., skip_special_tokens=True)` of one row: the ids below 3 (pad, EOS, unk) and
+    from 259 on (the `<extra_id_N>` sentinels) are dropped, every other id is the byte id - 3, and the bytes are
+    decoded as UTF-8 with `errors="ignore"`."""
+    data = bytes(int(i) - BYTE_OFFSET for i in ids if BYTE_OFFSET <= int(i) < BYTE_OFFSET + VOCAB_BYTES)
+    return data.decode("utf-8", errors="ignore")
