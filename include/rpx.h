@@ -433,13 +433,16 @@ int rpx_gemm_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, i
 int rpx_gemm1_bf16_f32(const void* d_A, const void* d_B, float* d_C, int32_t M, int32_t N,
                        int32_t K, void* stream);
 
-enum { RPX_EGEMM_QKV = 0, RPX_EGEMM_OPROJ = 1, RPX_EGEMM_FFN_UP = 2, RPX_EGEMM_FFN_DOWN = 3 };
+enum { RPX_EGEMM_QKV = 0, RPX_EGEMM_OPROJ = 1, RPX_EGEMM_FFN_UP = 2, RPX_EGEMM_FFN_DOWN = 3, RPX_EGEMM_HEAD = 4 };
 /* One encoder GEMM, launched as the forward pass launches it for T tokens on the throughput (latency = 0) or
  * latency path, PDL scope set as forward() sets it for that T.  A [T, K] bf16 (lda = K), B [N, K] bf16 in the
- * packed layout rpx_encoder_create writes.  D = d_model = K for QKV / FFN-up, N for O-proj / FFN-down.
+ * packed layout rpx_encoder_create writes.  D = d_model = K for QKV / FFN-up / HEAD, N for O-proj / FFN-down.
  *   QKV     out [T, N] bf16 = bf16(A B^T * rs[m]),  rs from ss_in
  *   FFN_UP  out [T, N/2] bf16 gated GELU,             rs from ss_in;  N % 256 == 0
  *   OPROJ / FFN_DOWN   h32 [T, N] += A B^T;  h16 = bf16(h32);  ss_out partials
+ *   HEAD    out [T, N] fp32 = A B^T * rs[m], the generator's output head, rs from ss_in;  N % 32 == 0.  It runs on
+ *           the throughput core on both paths (as in the teacher-forced forward and in every decode step);
+ *           `latency` selects only the layout of ss_in.
  * ss_in / ss_out: [parts][T] fp32, parts = ceil(D / 128) (throughput) or D / 32 (latency).
  * d_prefetch (latency QKV only, else NULL): prefetch_bytes fetched into L2 by the CTAs the GEMM leaves idle. */
 int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const void* d_B, int32_t T,
@@ -491,6 +494,21 @@ int rpx_debug_attention_ex(int32_t mode, const void* d_q, const void* d_kv, void
 int rpx_debug_decode_attention(const void* d_cache, const int32_t* d_lin, const float* d_lut, void* d_out, int32_t t,
                                int32_t rows, int32_t max_length, int32_t n_heads, int32_t rel_max_distance,
                                void* stream);
+
+/* The search half of rpx_seq2seq_generate on caller-supplied logits, for tests: the same init, step and finish
+ * kernels with the same arguments, under the same checks (vocab in place of the decoder's vocab_size), with no
+ * decoder or encoder.
+ *   d_logits  fp32 [max_length - 1][batch * num_beams][vocab]: step t reads slab t as the decoder's logits of the
+ *             rows' current tokens (row b * num_beams + j is beam j of state b)
+ *   start_id  the decoder start id (also the pad id, as rpx_t5_decoder_create requires)
+ * Outputs and the optional trace are those of rpx_seq2seq_generate; *h_steps is the step at which the last search
+ * ended.  Every step runs (a state whose search is done returns at once from each later one).  Synchronises
+ * `stream`. */
+size_t rpx_debug_search_workspace_bytes(int32_t batch, int32_t num_beams, int32_t max_length);
+int rpx_debug_search(const float* d_logits, int32_t batch, int32_t num_beams, int32_t vocab, int32_t num_return,
+                     int32_t max_length, double length_penalty, int32_t eos_id, int32_t start_id,
+                     int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                     const rpx_generate_trace* trace, void* d_workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

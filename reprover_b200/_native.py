@@ -146,6 +146,10 @@ _SIGNATURES = {
                                        C.POINTER(C.c_int32), C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_debug_decode_attention": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                              C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    "rpx_debug_search_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "rpx_debug_search": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                   C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32),
+                                   C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "rpx_encoder_set_debug_hidden": (C.c_int, [C.c_void_p, C.c_void_p]),
     "rpx_encoder_set_profiling": (C.c_int, [C.c_void_p, C.c_int32]),
     "rpx_encoder_read_profile": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64)]),
@@ -196,6 +200,7 @@ RPX_EGEMM_QKV = 0
 RPX_EGEMM_OPROJ = 1
 RPX_EGEMM_FFN_UP = 2
 RPX_EGEMM_FFN_DOWN = 3
+RPX_EGEMM_HEAD = 4
 
 RPX_ATTN_BIDIRECTIONAL = 0
 RPX_ATTN_CAUSAL = 1

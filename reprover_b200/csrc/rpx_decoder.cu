@@ -317,11 +317,9 @@ int decoder_layer(const rpx_t5_decoder* d, const DecLayerW& w, int layer, const 
 // ---------------------------------------------------------------------------------------------- generate
 // The search half over B states, nb beams, R = B nb rows.  Nothing here grows with the step: the KV cache holds
 // every step's q | k | v rows in place, [num_layers][max_length][R][3 inner] bf16.
-struct GenWs {
-  size_t dec_off;
-  __nv_bfloat16* cross_kv;  // the prefill's
-  __nv_bfloat16* cache;
-  float* logits;            // [R, vocab]
+
+// The search's own state: what the init, step and finish kernels read and write besides the logits.
+struct SearchBufs {
   int32_t* tokens;          // [max_length][R]
   int32_t* lin;             // [2][R][max_length]
   float* run_score;         // [R]
@@ -331,6 +329,28 @@ struct GenWs {
   int32_t* fin_seq;         // [2][R][max_length]
   int32_t* state;           // [B][4]
   int32_t* counters;        // done count, out_len, last step
+};
+
+SearchBufs carve_search(Carver& c, int64_t B, int64_t R, int64_t ML) {
+  SearchBufs s{};
+  s.tokens = (int32_t*)c.take((size_t)ML * R * 4);
+  s.lin = (int32_t*)c.take(2 * (size_t)R * ML * 4);
+  s.run_score = (float*)c.take((size_t)R * 4);
+  s.fin_score = (float*)c.take(2 * (size_t)R * 4);
+  s.fin_len = (int32_t*)c.take(2 * (size_t)R * 4);
+  s.fin_flag = (int32_t*)c.take(2 * (size_t)R * 4);
+  s.fin_seq = (int32_t*)c.take(2 * (size_t)R * ML * 4);
+  s.state = (int32_t*)c.take((size_t)B * 16);
+  s.counters = (int32_t*)c.take(16);
+  return s;
+}
+
+struct GenWs {
+  size_t dec_off;
+  __nv_bfloat16* cross_kv;  // the prefill's
+  __nv_bfloat16* cache;
+  float* logits;            // [R, vocab]
+  SearchBufs s;
   size_t cache_layer;       // elements of one layer's cache
   size_t total;
 };
@@ -346,17 +366,44 @@ GenWs carve_gen(const rpx_t5_decoder* d, const rpx_encoder* e, uint8_t* base, __
   w.cache_layer = (size_t)ML * R * 3 * d->inner;
   w.cache = (__nv_bfloat16*)c.take(w.cache_layer * d->cfg.num_layers * 2);
   w.logits = (float*)c.take((size_t)R * d->cfg.vocab_size * 4);
-  w.tokens = (int32_t*)c.take((size_t)ML * R * 4);
-  w.lin = (int32_t*)c.take(2 * (size_t)R * ML * 4);
-  w.run_score = (float*)c.take((size_t)R * 4);
-  w.fin_score = (float*)c.take(2 * (size_t)R * 4);
-  w.fin_len = (int32_t*)c.take(2 * (size_t)R * 4);
-  w.fin_flag = (int32_t*)c.take(2 * (size_t)R * 4);
-  w.fin_seq = (int32_t*)c.take(2 * (size_t)R * ML * 4);
-  w.state = (int32_t*)c.take((size_t)B * 16);
-  w.counters = (int32_t*)c.take(16);
+  w.s = carve_search(c, B, R, ML);
   w.total = c.off;
   return w;
+}
+
+// The search's three launches, shared by search() and rpx_debug_search so that both run the same kernels with the
+// same arguments.  A search over B states of nb beams (R = B nb rows; greedy: nb = 1, one state per row).
+struct SearchShape {
+  int B, nb, V, ML;
+  int rows() const { return B * nb; }
+  int states() const { return nb > 1 ? B : rows(); }  // greedy: one state per row
+};
+
+int search_init(const SearchBufs& s, const SearchShape& sh, int start_id, cudaStream_t st) {
+  const int R = sh.rows(), nb = sh.nb;
+  GenerateInitArgs ia{s.tokens, nb > 1 ? s.lin : nullptr, s.run_score, s.fin_score, s.fin_len, s.fin_flag, s.state,
+                      s.counters, s.counters + 1, s.counters + 2, R, sh.states(), nb, sh.ML, start_id};
+  return launch_generate_init(ia, st);
+}
+
+// Step t on logits [R, V]; the trace, if any, records it while t < trace->max_steps.
+int search_step(const SearchBufs& s, const SearchShape& sh, const float* logits, double length_penalty, int eos_id,
+                const rpx_generate_trace* trace, int t, cudaStream_t st) {
+  const int R = sh.rows(), V = sh.V;
+  const bool tr = trace && t < trace->max_steps;
+  BeamStepArgs sa{logits, s.tokens, s.lin, s.run_score, s.fin_score, s.fin_len, s.fin_flag, s.fin_seq, s.state,
+                  s.counters, s.counters + 2, tr ? trace->d_scores + (size_t)t * R * V : nullptr,
+                  tr ? trace->d_parents + (size_t)t * R : nullptr, tr ? trace->d_tokens + (size_t)t * R : nullptr,
+                  (float)pow((double)(t + 1), length_penalty), t, R, sh.nb, V, sh.ML, eos_id};
+  return launch_search_step(sa, sh.states(), st);
+}
+
+int search_finish(const SearchBufs& s, const SearchShape& sh, int num_return, int start_id, int eos_id,
+                  int64_t* d_sequences, float* d_scores, cudaStream_t st) {
+  const int nb = sh.nb;
+  GenerateFinishArgs fa{s.tokens, s.fin_score, s.fin_len, s.fin_seq, s.state, d_sequences, d_scores, s.counters + 1,
+                        sh.rows(), nb, num_return, sh.ML, start_id, nb > 1 && start_id == 0 ? eos_id : start_id};
+  return launch_generate_finish(fa, sh.states(), st);
 }
 
 // One decoder step for all R rows at position t: embed the rows' current tokens, every layer on the latency-path
@@ -367,7 +414,7 @@ int decode_step(const rpx_t5_decoder* d, const rpx_encoder* e, const GenWs& g, c
   const rpx_t5_config& c = d->cfg;
   const int R = B * nb, D = c.d_model, inner = d->inner, F = c.d_ff, P = e->n_parts_lat;
   const float inv_d = 1.0f / (float)D;
-  RPX_TRY(launch_embed(g.tokens + (size_t)t * R, d->emb, dw.h32, dw.h16, dw.ssA, R, P, R, D, st));
+  RPX_TRY(launch_embed(g.s.tokens + (size_t)t * R, d->emb, dw.h32, dw.h16, dw.ssA, R, P, R, D, st));
   float* sa = dw.ssA;
   float* sb = dw.ssB;
   for (int l = 0; l < c.num_layers; ++l) {
@@ -375,8 +422,8 @@ int decode_step(const rpx_t5_decoder* d, const rpx_encoder* e, const GenWs& g, c
     __nv_bfloat16* cache = g.cache + g.cache_layer * l;
     RPX_TRY(qkv_gemm(true, R, dw.h16, w.qkv, 3 * inner, D, RowScale{sa, P, R, inv_d, c.ln_eps},
                      cache + (size_t)t * R * 3 * inner, nullptr, 0, st));
-    DecodeAttnArgs da{cache, nb > 1 ? g.lin + (size_t)(t & 1) * R * ML : nullptr, d->bias_lut, dw.attn, g.state, t, R,
-                      3 * inner, inner, c.num_heads, ML, c.rel_max_distance, nb};
+    DecodeAttnArgs da{cache, nb > 1 ? g.s.lin + (size_t)(t & 1) * R * ML : nullptr, d->bias_lut, dw.attn, g.s.state,
+                      t, R, 3 * inner, inner, c.num_heads, ML, c.rel_max_distance, nb};
     RPX_TRY(launch_decode_attention(da, st));
     RPX_TRY(oproj_gemm(true, R, dw.attn, w.o, D, inner, dw.h32, dw.h16, sb, st));
     RPX_TRY(qkv_gemm(true, R, dw.h16, w.cq, inner, D, RowScale{sb, P, R, inv_d, c.ln_eps}, dw.qkv, nullptr, 0, st));
@@ -390,8 +437,7 @@ int decode_step(const rpx_t5_decoder* d, const rpx_encoder* e, const GenWs& g, c
     sa = sb;
     sb = tmp;
   }
-  EpiWsStoreF32Scaled::Params ep{g.logits, c.vocab_size, RowScale{sa, P, R, inv_d, c.ln_eps}};
-  return launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(dw.h16, D, d->head, D, R, c.vocab_size, D, ep, st);
+  return head_gemm(R, dw.h16, d->head, c.vocab_size, D, RowScale{sa, P, R, inv_d, c.ln_eps}, g.logits, st);
 }
 
 // Steps enqueued between two reads of the done-state count.
@@ -539,8 +585,8 @@ int teacher_forced(const rpx_t5_decoder* dec, const rpx_encoder* enc, const Pref
       RPX_TRY(decoder_layer(dec, dec->layers[l], l, dw, T_dec, B, p.max_dec, cross_kv, T_enc, p.ew.cu_tokens, &ss_in,
                             &ss_other, st));
     // ---- head
-    EpiWsStoreF32Scaled::Params ep{sw.logits, V, RowScale{ss_in, P, T_dec, 1.0f / (float)D, c.ln_eps}};
-    RPX_TRY((launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(dw.h16, D, dec->head, D, T_dec, V, D, ep, st)));
+    RPX_TRY(head_gemm(T_dec, dw.h16, dec->head, V, D, RowScale{ss_in, P, T_dec, 1.0f / (float)D, c.ln_eps}, sw.logits,
+                      st));
     token_logprob_kernel<<<ceil_div(T_dec, 8), 256, 0, st>>>(sw.logits, sw.targets, sw.tok_lp, T_dec, V);
     RPX_CUDA_OK(cudaGetLastError());
   }
@@ -562,17 +608,16 @@ int teacher_forced(const rpx_t5_decoder* dec, const rpx_encoder* enc, const Pref
 int search(rpx_t5_decoder* dec, const rpx_encoder* enc, const Prefill& p, uint8_t* base, const GenWs& g, int B, int nb,
            int num_return, int ML, double length_penalty, int eos_id, int64_t* d_sequences, float* d_scores,
            const rpx_generate_trace* trace, cudaStream_t st) {
-  const int R = B * nb, V = dec->cfg.vocab_size;
+  const int R = B * nb;
+  const SearchShape sh{B, nb, dec->cfg.vocab_size, ML};
   const Workspace dw = carve(enc, base + g.dec_off, R, B);
   int32_t* cu_beam = dec->h_cu.data() + 2 * B + 2;  // the beams' query offsets, b nb
   for (int b = 0; b <= B; ++b) cu_beam[b] = b * nb;
   RPX_CUDA_OK(cudaMemcpyAsync(dw.cu_tokens, cu_beam, ((size_t)B + 1) * 4, cudaMemcpyHostToDevice, st));
-  GenerateInitArgs ia{g.tokens, nb > 1 ? g.lin : nullptr, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.state,
-                      g.counters, g.counters + 1, g.counters + 2, R, nb > 1 ? B : R, nb, ML, dec->start_id};
-  RPX_TRY(launch_generate_init(ia, st));
+  RPX_TRY(search_init(g.s, sh, dec->start_id, st));
 
   // ---- the steps, enqueued in blocks; the done-state count of the block before is read while a block runs
-  const int states = nb > 1 ? B : R;
+  const int states = sh.states();
   int t = 0, blk = 0;
   {
     PdlScope pdl_scope(true);
@@ -580,14 +625,9 @@ int search(rpx_t5_decoder* dec, const rpx_encoder* enc, const Prefill& p, uint8_
       const int t_end = t + kPollSteps < ML - 1 ? t + kPollSteps : ML - 1;
       for (; t < t_end; ++t) {
         RPX_TRY(decode_step(dec, enc, g, dw, p.ew.cu_tokens, p.T_enc, B, nb, ML, t, st));
-        const bool tr = trace && t < trace->max_steps;
-        BeamStepArgs sa{g.logits, g.tokens, g.lin, g.run_score, g.fin_score, g.fin_len, g.fin_flag, g.fin_seq, g.state,
-                        g.counters, g.counters + 2, tr ? trace->d_scores + (size_t)t * R * V : nullptr,
-                        tr ? trace->d_parents + (size_t)t * R : nullptr, tr ? trace->d_tokens + (size_t)t * R : nullptr,
-                        (float)pow((double)(t + 1), length_penalty), t, R, nb, V, ML, eos_id};
-        RPX_TRY(launch_search_step(sa, states, st));
+        RPX_TRY(search_step(g.s, sh, g.logits, length_penalty, eos_id, trace, t, st));
       }
-      RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + (blk & 1), g.counters, 4, cudaMemcpyDeviceToHost, st));
+      RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + (blk & 1), g.s.counters, 4, cudaMemcpyDeviceToHost, st));
       RPX_CUDA_OK(cudaEventRecord(dec->poll_ev[blk & 1], st));
       if (blk > 0) {
         RPX_CUDA_OK(cudaEventSynchronize(dec->poll_ev[(blk - 1) & 1]));
@@ -596,12 +636,10 @@ int search(rpx_t5_decoder* dec, const rpx_encoder* enc, const Prefill& p, uint8_
       ++blk;
     }
   }
-  GenerateFinishArgs fa{g.tokens, g.fin_score, g.fin_len, g.fin_seq, g.state, d_sequences, d_scores, g.counters + 1, R,
-                        nb, num_return, ML, dec->start_id, nb > 1 && dec->start_id == 0 ? eos_id : dec->start_id};
-  RPX_TRY(launch_generate_finish(fa, nb > 1 ? B : R, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 2, g.counters + 1, 4, cudaMemcpyDeviceToHost, st));
+  RPX_TRY(search_finish(g.s, sh, num_return, dec->start_id, eos_id, d_sequences, d_scores, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 2, g.s.counters + 1, 4, cudaMemcpyDeviceToHost, st));
   RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 3, p.ew.flag, 4, cudaMemcpyDeviceToHost, st));
-  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 4, g.counters + 2, 4, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaMemcpyAsync(dec->h_poll + 4, g.s.counters + 2, 4, cudaMemcpyDeviceToHost, st));
   RPX_CUDA_OK(cudaStreamSynchronize(st));
   return RPX_OK;
 }
@@ -860,6 +898,45 @@ int rpx_debug_decode_attention(const void* d_cache, const int32_t* d_lin, const 
   DecodeAttnArgs a{static_cast<const __nv_bfloat16*>(d_cache), d_lin, d_lut, static_cast<__nv_bfloat16*>(d_out), nullptr,
                    t, rows, 3 * inner, inner, n_heads, max_length, rel_max_distance, 1};
   return launch_decode_attention(a, static_cast<cudaStream_t>(stream));
+}
+
+size_t rpx_debug_search_workspace_bytes(int32_t batch, int32_t num_beams, int32_t max_length) {
+  if (batch <= 0 || num_beams <= 0 || num_beams > kMaxBeams || max_length < 2) return 0;
+  Carver c{nullptr};
+  carve_search(c, batch, (int64_t)batch * num_beams, max_length);
+  return c.off;
+}
+
+int rpx_debug_search(const float* d_logits, int32_t batch, int32_t num_beams, int32_t vocab, int32_t num_return,
+                     int32_t max_length, double length_penalty, int32_t eos_id, int32_t start_id,
+                     int64_t* d_sequences, float* d_scores, int32_t* h_out_len, int32_t* h_steps,
+                     const rpx_generate_trace* trace, void* d_workspace, size_t workspace_bytes, void* stream) {
+  RPX_REQUIRE(d_logits && d_sequences && h_out_len && d_workspace, RPX_ERR_INVALID, "rpx_debug_search: null argument");
+  RPX_REQUIRE(vocab > 0, RPX_ERR_INVALID, "rpx_debug_search: vocab=%d", vocab);
+  RPX_TRY(check_gen_args("rpx_debug_search", batch, 1, num_beams, num_return, max_length, eos_id, d_scores, vocab));
+  RPX_REQUIRE(start_id >= 0 && start_id < vocab, RPX_ERR_INVALID, "rpx_debug_search: start_id=%d outside [0, %d)",
+              start_id, vocab);
+  RPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, RPX_ERR_INVALID, "workspace must be 256-byte aligned");
+  RPX_REQUIRE(!trace || (trace->d_scores && trace->d_parents && trace->d_tokens && trace->max_steps >= 0),
+              RPX_ERR_INVALID, "rpx_debug_search: incomplete trace");
+  const int64_t R = (int64_t)batch * num_beams;
+  Carver c{static_cast<uint8_t*>(d_workspace)};
+  const SearchBufs s = carve_search(c, batch, R, max_length);
+  RPX_REQUIRE(c.off <= workspace_bytes, RPX_ERR_WORKSPACE, "workspace too small: need %zu, have %zu", c.off,
+              workspace_bytes);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RPX_TRY(configure_search_step(kMaxStepSmem));
+  const SearchShape sh{batch, num_beams, vocab, max_length};
+  RPX_TRY(search_init(s, sh, start_id, st));
+  for (int t = 0; t < max_length - 1; ++t)
+    RPX_TRY(search_step(s, sh, d_logits + (size_t)t * R * vocab, length_penalty, eos_id, trace, t, st));
+  RPX_TRY(search_finish(s, sh, num_return, start_id, eos_id, d_sequences, d_scores, st));
+  int32_t counters[3];
+  RPX_CUDA_OK(cudaMemcpyAsync(counters, s.counters, sizeof counters, cudaMemcpyDeviceToHost, st));
+  RPX_CUDA_OK(cudaStreamSynchronize(st));
+  *h_out_len = counters[1];
+  if (h_steps) *h_steps = counters[2];
+  return RPX_OK;
 }
 
 int rpx_debug_attention_ex(int32_t mode, const void* d_q, const void* d_kv, void* d_out, const int32_t* d_cu_q,

@@ -308,6 +308,14 @@ int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K,
   return launch_gemm<128, EpiGeGLUT<64>, false, kGemmStages, true>(A, K, B, K, T, N, K, ep, st);
 }
 
+// out [T, N] fp32 = A B^T * rs[m].  The generator's output head (rpx_decoder.cu), on the throughput core in both the
+// teacher-forced forward and every decode step; only the layout of the partial sums behind rs differs.  ByT5's
+// N = 384 ends in a 128-column n-tile.
+int head_gemm(int T, const void* A, const void* B, int N, int K, const RowScale& rs, float* out, cudaStream_t st) {
+  EpiWsStoreF32Scaled::Params ep{out, N, rs};
+  return launch_gemm_ws<EpiWsStoreF32Scaled, 4, 2>(A, K, B, K, T, N, K, ep, st);
+}
+
 namespace {
 
 // One encoder block on the throughput or the latency path, each kernel under its profiling class.
@@ -620,7 +628,7 @@ int rpx_encoder_set_profiling(rpx_encoder* enc, int32_t enable) {
 int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const void* d_B, int32_t T, int32_t N,
                            int32_t K, float ln_eps, const float* d_ss_in, void* d_out, float* d_h32, void* d_h16,
                            float* d_ss_out, const void* d_prefetch, size_t prefetch_bytes, void* stream) {
-  RPX_REQUIRE(site >= RPX_EGEMM_QKV && site <= RPX_EGEMM_FFN_DOWN, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: site=%d", site);
+  RPX_REQUIRE(site >= RPX_EGEMM_QKV && site <= RPX_EGEMM_HEAD, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: site=%d", site);
   RPX_REQUIRE(d_A && d_B, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: null operand");
   RPX_REQUIRE(T > 0 && N > 0 && K > 0, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: T=%d N=%d K=%d", T, N, K);
   const bool lat = latency != 0;
@@ -631,6 +639,8 @@ int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const
     RPX_REQUIRE(d_h32 && d_h16 && d_ss_out, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: residual site needs h32, h16, ss_out");
   else
     RPX_REQUIRE(d_ss_in && d_out, RPX_ERR_INVALID, "rpx_debug_encoder_gemm: site %d needs ss_in and out", site);
+  if (site == RPX_EGEMM_HEAD)
+    RPX_REQUIRE(N % 32 == 0, RPX_ERR_UNSUPPORTED, "rpx_debug_encoder_gemm: head N=%d must be a multiple of 32", N);
   RPX_REQUIRE(d_prefetch == nullptr || (lat && site == RPX_EGEMM_QKV), RPX_ERR_INVALID,
               "rpx_debug_encoder_gemm: only the latency QKV projection prefetches");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -642,6 +652,7 @@ int rpx_debug_encoder_gemm(int32_t site, int32_t latency, const void* d_A, const
     case RPX_EGEMM_QKV: return qkv_gemm(lat, T, d_A, d_B, N, K, rs, out, d_prefetch, prefetch_bytes, st);
     case RPX_EGEMM_OPROJ: return oproj_gemm(lat, T, d_A, d_B, N, K, d_h32, h16, d_ss_out, st);
     case RPX_EGEMM_FFN_UP: return ffn_up_gemm(lat, T, d_A, d_B, N, K, rs, out, st);
+    case RPX_EGEMM_HEAD: return head_gemm(T, d_A, d_B, N, K, rs, static_cast<float*>(d_out), st);
     default: return ffn_down_gemm(lat, T, d_A, d_B, N, K, d_h32, h16, d_ss_out, st);
   }
 }

@@ -1,5 +1,5 @@
 // rpx_encoder.cuh — the encoder's handle and the parts of its forward pass (rpx_encoder.cu) that the generator's
-// decoder (rpx_decoder.cu) runs as well: the workspace, the four GEMM launchers, the bias table, forward().
+// decoder (rpx_decoder.cu) runs as well: the workspace, the GEMM launchers, the bias table, forward().
 #pragma once
 #include <vector>
 
@@ -100,6 +100,8 @@ int ffn_down_gemm(bool latency, int T, const void* A, const void* B, int N, int 
                   float* ss_out, cudaStream_t st);
 int ffn_up_gemm(bool latency, int T, const void* A, const void* B, int N, int K, const RowScale& rs,
                 __nv_bfloat16* out, cudaStream_t st);
+// The generator's output head: out [T, N] fp32 = A B^T * rs[m], always on the throughput core.
+int head_gemm(int T, const void* A, const void* B, int N, int K, const RowScale& rs, float* out, cudaStream_t st);
 
 // What forward() writes after the last block.
 //   kPooled    final RMSNorm + masked mean + L2 normalise: [S, D]

@@ -367,19 +367,27 @@ __global__ void __launch_bounds__(kStepThreads) beam_step_kernel(BeamStepArgs a)
   }
 }
 
-// num_beams == 1 (HF greedy `_sample`): one CTA per row, argmax of the fp32 logits (lowest id on ties); the row is
-// done at EOS or max_length, and its later tokens are the pad id (the finishing kernel writes them).
+// (v, j) comes before (best, arg) in torch.argmax's order: a NaN above every number (the first NaN wins), then the
+// larger value, then the lower id.
+__device__ __forceinline__ bool argmax_before(float v, int j, float best, int arg) {
+  if (isnan(v)) return !isnan(best) || j < arg;
+  return v > best || (v == best && j < arg);
+}
+
+// num_beams == 1 (HF greedy `_sample`): one CTA per row, torch.argmax of the fp32 logits (the lowest id of the
+// maximum; the first NaN if the row holds one); the row is done at EOS or max_length, and its later tokens are the
+// pad id (the finishing kernel writes them).
 __global__ void __launch_bounds__(256) greedy_step_kernel(BeamStepArgs a) {
   const int r = blockIdx.x;
   int32_t* st = a.state + 4 * r;
   if (st[0] != 0) return;
   const float* x = a.logits + (size_t)r * a.vocab;
   float best = -INFINITY;
-  int arg = 0x7fffffff;
+  int arg = 0x7fffffff;  // any id of the row comes before it, -inf included
   for (int j = threadIdx.x; j < a.vocab; j += blockDim.x) {
     const float v = x[j];
     if (a.trace_scores) a.trace_scores[(size_t)r * a.vocab + j] = v;
-    if (v > best || (v == best && j < arg)) {
+    if (argmax_before(v, j, best, arg)) {
       best = v;
       arg = j;
     }
@@ -389,7 +397,7 @@ __global__ void __launch_bounds__(256) greedy_step_kernel(BeamStepArgs a) {
   for (int off = 16; off; off >>= 1) {
     const float ov = __shfl_xor_sync(kFullMask, best, off);
     const int oi = __shfl_xor_sync(kFullMask, arg, off);
-    if (ov > best || (ov == best && oi < arg)) {
+    if (argmax_before(ov, oi, best, arg)) {
       best = ov;
       arg = oi;
     }
@@ -401,11 +409,10 @@ __global__ void __launch_bounds__(256) greedy_step_kernel(BeamStepArgs a) {
   __syncthreads();
   if (threadIdx.x == 0) {
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
-      if (bv[w] > best || (bv[w] == best && bi[w] < arg)) {
+      if (argmax_before(bv[w], bi[w], best, arg)) {
         best = bv[w];
         arg = bi[w];
       }
-    if (arg >= a.vocab) arg = 0;  // all-NaN row: HF's argmax would return the first NaN; the id is 0 here
     a.tokens[(size_t)(a.t + 1) * a.rows + r] = arg;
     a.fin_len[r] = a.t + 1;
     if (a.trace_parents) {

@@ -4,6 +4,16 @@ asc).  `tests/test_generate_cpu.py` pins it against HF `generate`; the GPU tests
 log-probs, so the search bookkeeping is checked apart from the arithmetic.
 
     step_fn(t, prefixes [R, t + 1] int64) -> fp32 [R, V]   log-probs (beam search) or logits (greedy)
+
+`beam_search(defect=...)` plants one bookkeeping mistake a step kernel could make (default None: none), so that
+tests/test_search_cases_cpu.py can show that the constructed cases of tests/search_cases.py tell it apart:
+
+    thr_high_index       of the keys equal to the 2 nb-th largest, those of the highest flat indices are taken
+    run_desc             the running choice breaks ties by descending position
+    merge_cand_first     the finished merge ranks the step's candidates before the kept hypotheses on ties
+    penalty_at_t         finished scores divided by t ** lp instead of (t + 1) ** lp (1 at t = 0)
+    heuristic_prev       the early-stop heuristic tests the finished set of the step before
+    fin_wrong_lineage    a finished hypothesis copies its tokens from the next beam's row, not its parent's
 """
 from __future__ import annotations
 
@@ -15,10 +25,28 @@ import torch
 MASK = -1.0e9
 
 
+DEFECTS = ("thr_high_index", "run_desc", "merge_cand_first", "penalty_at_t", "heuristic_prev", "fin_wrong_lineage")
+
+
 def _topk(x: torch.Tensor, k: int):
     """torch.topk along the last dim with ties by index ascending."""
     vals, idx = torch.sort(x, dim=-1, descending=True, stable=True)
     return vals[..., :k], idx[..., :k]
+
+
+def _topk_desc(x: torch.Tensor, k: int):
+    """torch.topk along the last dim with ties by index descending."""
+    n = x.shape[-1]
+    vals, idx = torch.sort(x.flip(-1), dim=-1, descending=True, stable=True)
+    return vals[..., :k], (n - 1 - idx)[..., :k]
+
+
+def _topk_thr_high(x: torch.Tensor, k: int):
+    """The k largest with the ties at the k-th value taken from the highest indices, then ranked (value desc, index
+    asc) like _topk."""
+    sel = _topk_desc(x, k)[1].sort(-1).values
+    vals, order = torch.sort(torch.gather(x, -1, sel), dim=-1, descending=True, stable=True)
+    return vals, torch.gather(sel, -1, order)
 
 
 def _gather(t: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
@@ -50,8 +78,10 @@ def _gap(sorted_vals: torch.Tensor, i: int) -> float:
 
 
 def beam_search(step_fn: Callable, batch: int, num_beams: int, num_return: int, max_length: int,
-                length_penalty: float, eos: int, pad: int, start: int, stats: Optional[SearchStats] = None):
+                length_penalty: float, eos: int, pad: int, start: int, stats: Optional[SearchStats] = None,
+                defect: Optional[str] = None):
     """(sequences [batch * num_return, L_out] int64, sequences_scores [batch * num_return] fp32)."""
+    assert defect is None or defect in DEFECTS, defect
     B, nb = batch, num_beams
     fill = pad or eos
     cur_len = 1
@@ -74,7 +104,7 @@ def beam_search(step_fn: Callable, batch: int, num_beams: int, num_return: int, 
         V = lp.shape[-1]
         lp = lp.view(B, nb, V) + running_scores[:, :, None]
         lp = lp.reshape(B, nb * V)
-        top_lp, top_idx = _topk(lp, 2 * nb)
+        top_lp, top_idx = (_topk_thr_high if defect == "thr_high_index" else _topk)(lp, 2 * nb)
         live = unsat[:, 0].clone()
         n_terms = t + 1                                 # log-probs summed into a running score
         fin_terms = n_terms ** (1 - length_penalty)     # ... their weight in a length-penalised score
@@ -85,7 +115,7 @@ def beam_search(step_fn: Callable, batch: int, num_beams: int, num_return: int, 
         hits = (tok == eos) | (cur_len + 1 >= max_length)
         # running beams for the next step
         run_lp = top_lp + hits.to(torch.float32) * MASK
-        nxt = _topk(run_lp, nb)[1]
+        nxt = (_topk_desc if defect == "run_desc" else _topk)(run_lp, nb)[1]
         for b in range(B):
             if live[b]:
                 margin[b] = min(margin[b], _gap(_topk(run_lp[b], 2 * nb)[0], nb - 1) / n_terms)
@@ -93,18 +123,28 @@ def beam_search(step_fn: Callable, batch: int, num_beams: int, num_return: int, 
         new_running_scores = _gather(run_lp, nxt)
         # finished beams
         did = hits & top_mask[None, :]
-        fin = top_lp / ((cur_len + 1 - 1) ** length_penalty)
+        pen_len = max(cur_len - 1, 1) if defect == "penalty_at_t" else cur_len + 1 - 1
+        fin = top_lp / (pen_len ** length_penalty)
         fin += (~unsat).to(torch.float32) * MASK
         fin += (~did) * MASK
         for b in range(B):
             for c in range(nb):
                 if did[b, c] and unsat[b, 0]:
                     stats.finish_lengths.add(cur_len)
-        merged_seq = torch.cat([sequences, top_seq], 1)
+        fin_seq = top_seq
+        if defect == "fin_wrong_lineage":
+            fin_seq = _gather(running, (parent + 1) % nb)
+            fin_seq[:, :, cur_len] = tok
+        merged_seq = torch.cat([sequences, fin_seq], 1)
         merged_scores = torch.cat([beam_scores, fin], 1)
         merged_fin = torch.cat([is_finished, did], 1)
         merged_len = torch.cat([gen_len, torch.full((B, 2 * nb), cur_len)], 1)
-        keep = _topk(merged_scores, nb)[1]
+        if defect == "merge_cand_first":  # the candidates first: position order [candidates, kept]
+            perm = torch.cat([torch.arange(nb, 3 * nb), torch.arange(nb)])
+            keep = perm[_topk(merged_scores[:, perm], nb)[1]]
+        else:
+            keep = _topk(merged_scores, nb)[1]
+        prev_scores, prev_finished = beam_scores, is_finished
         for b in range(B):
             if live[b]:
                 margin[b] = min(margin[b], _gap(_topk(merged_scores[b], 3 * nb)[0], nb - 1) / fin_terms)
@@ -116,7 +156,10 @@ def beam_search(step_fn: Callable, batch: int, num_beams: int, num_return: int, 
         cur_len += 1
         t += 1
         best = running_scores[:, :1] / ((cur_len - 1) ** length_penalty)
-        worst = torch.where(is_finished, torch.min(beam_scores, dim=1, keepdim=True)[0], MASK)
+        if defect == "heuristic_prev":
+            worst = torch.where(prev_finished, torch.min(prev_scores, dim=1, keepdim=True)[0], MASK)
+        else:
+            worst = torch.where(is_finished, torch.min(beam_scores, dim=1, keepdim=True)[0], MASK)
         new_unsat = unsat & torch.any(best > worst, dim=-1, keepdim=True)
         for b in range(B):
             if live[b] and bool(is_finished[b].all()):

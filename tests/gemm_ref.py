@@ -59,6 +59,11 @@ FFN-up     x = fl(g * rs_k), y = fl(l * rs_k) with g, l the gate and linear accu
            dg = GELU_LIP dx + (|x| + dx)/2 (dt_arith (1 + ETA) + ETA + 4u);
            out = fl(gelu * y): tol = dg (|y| + dy) + |gelu| dy + u (|gelu| + dg)(|y| + dy).
 
+Head       out = fl(acc * rs_k) in fp32, the generator's output head: the bound of QKV (whose u term is that
+           product's rounding) plus one more fp32 rounding, u (|ref| + tol), which also covers the float64
+           reference's own rounding; |out - ref| <= tol directly, with no bf16 bracket.  Row chunks hold at most
+           2^24 outputs, so a 32128-column vocabulary's float64 reference fits in memory at any T.
+
 Residual   h32_out = fl(h32_in + acc): |h32_out - (h32_in + E)| <= gamma S + u (|h32_in + E| + gamma S).
 (O-proj,   h16_out must equal bf16_rn(h32_out) bit for bit, from the kernel's own h32_out.
 FFN-down)  ss_out[p][m] is compared with the float64 sum of h32_out[m, c]^2 over exactly the columns c of part p
@@ -204,6 +209,34 @@ def check_qkv(out: torch.Tensor, A: torch.Tensor, B: torch.Tensor, ss_in: torch.
         n_boundary += int((o.double() != ref.float().to(torch.bfloat16).double()).sum())
     if stats is not None:
         stats.update(gamma=g, eps_rs=e_rs, n_not_rn_of_ref=n_boundary)
+    return f
+
+
+def check_head(out: torch.Tensor, A: torch.Tensor, B: torch.Tensor, ss_in: torch.Tensor, d_model: int, eps: float,
+               stats: dict | None = None) -> Findings:
+    """out [T, N] fp32 = A B^T * rs[m]."""
+    T, K = A.shape
+    N = B.shape[0]
+    g = gamma_acc(K)
+    e_rs = eps_rowscale(ss_in.shape[0])
+    f = Findings("head.out")
+    worst = 0.0
+    rows = max(1, min(ROW_CHUNK, (1 << 24) // N))
+    for r0 in range(0, T, rows):
+        r1 = min(T, r0 + rows)
+        E, S = accumulate(A[r0:r1], B)
+        rs = rowscale(ss_in[:, r0:r1], d_model, eps)[:, None]
+        ref = E * rs
+        del E
+        tol = rs * (g * S + (ref.abs() / rs + g * S) * (e_rs + U))
+        del S
+        tol += U * (ref.abs() + tol)
+        o = out[r0:r1].double()
+        err = (o - ref).abs()
+        f.add(~(err <= tol), r0, o, ref, tol)
+        worst = max(worst, float((err / tol).nan_to_num(math.inf).max()))
+    if stats is not None:
+        stats.update(gamma=g, eps_rs=e_rs, max_err_over_tol=worst)
     return f
 
 

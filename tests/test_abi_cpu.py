@@ -80,9 +80,11 @@ def test_compute_fails_loudly_without_gpu(rpx_lib):
     assert rc == _native.RPX_ERR_CUDA and _native.last_error()
     rc = rpx_lib.rpx_gemm1_bf16_f32(buf, buf, buf, 128, 256, 64, None)
     assert rc == _native.RPX_ERR_CUDA and _native.last_error()
-    for site in (_native.RPX_EGEMM_QKV, _native.RPX_EGEMM_FFN_UP):
-        rc = rpx_lib.rpx_debug_encoder_gemm(site, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None)
-        assert rc == _native.RPX_ERR_CUDA and _native.last_error()
+    for site in (_native.RPX_EGEMM_QKV, _native.RPX_EGEMM_FFN_UP, _native.RPX_EGEMM_HEAD):
+        for latency in (0, 1):
+            rc = rpx_lib.rpx_debug_encoder_gemm(site, latency, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None,
+                                                None, 0, None)
+            assert rc == _native.RPX_ERR_CUDA and _native.last_error()
     for site in (_native.RPX_EGEMM_OPROJ, _native.RPX_EGEMM_FFN_DOWN):
         rc = rpx_lib.rpx_debug_encoder_gemm(site, 1, buf, buf, 4, 64, 128, 1e-6, None, None, buf, buf, buf, None, 0, None)
         assert rc == _native.RPX_ERR_CUDA and _native.last_error()
@@ -98,15 +100,61 @@ def test_compute_fails_loudly_without_gpu(rpx_lib):
 
 
 @needs_no_gpu
-def test_encoder_gemm_entry_rejects_bad_input_before_touching_a_device(rpx_lib):
+def test_encoder_gemm_entry_rejects_bad_site_and_input_before_touching_a_device(rpx_lib):
+    """Sites outside [RPX_EGEMM_QKV, RPX_EGEMM_HEAD] and incomplete arguments of every site are refused before any
+    CUDA call."""
     buf = (C.c_uint8 * 1024)()
     call = rpx_lib.rpx_debug_encoder_gemm
-    assert call(4, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(5, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(-1, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_HEAD, 1, buf, buf, 4, 384, 64, 1e-6, None, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_HEAD, 0, buf, buf, 4, 384, 64, 1e-6, buf, None, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
+    assert call(_native.RPX_EGEMM_HEAD, 1, buf, buf, 4, 384, 64, 1e-6, buf, buf, None, None, None, buf, 64, None) == _native.RPX_ERR_INVALID
+    rc = call(_native.RPX_EGEMM_HEAD, 0, buf, buf, 4, 400, 64, 1e-6, buf, buf, None, None, None, None, 0, None)
+    assert rc == _native.RPX_ERR_UNSUPPORTED and "multiple of 32" in _native.last_error()
     assert call(_native.RPX_EGEMM_QKV, 0, buf, buf, 4, 256, 64, 1e-6, None, buf, None, None, None, None, 0, None) == _native.RPX_ERR_INVALID
     assert call(_native.RPX_EGEMM_OPROJ, 1, buf, buf, 4, 64, 64, 1e-6, None, None, buf, buf, None, None, 0, None) == _native.RPX_ERR_INVALID
     assert call(_native.RPX_EGEMM_QKV, 0, buf, buf, 4, 256, 64, 1e-6, buf, buf, None, None, None, buf, 64, None) == _native.RPX_ERR_INVALID
     rc = call(_native.RPX_EGEMM_FFN_UP, 1, buf, buf, 4, 384, 64, 1e-6, buf, buf, None, None, None, None, 0, None)
     assert rc == _native.RPX_ERR_UNSUPPORTED and "multiple of 256" in _native.last_error()
+
+
+def test_search_workspace_bytes(rpx_lib):
+    """The search entry point's workspace: 0 outside the engine's ranges, and growing with batch, beams and length."""
+    ws = rpx_lib.rpx_debug_search_workspace_bytes
+    for bad in ((0, 4, 10), (2, 0, 10), (2, 129, 10), (2, 4, 1)):
+        assert ws(*bad) == 0, bad
+    assert 0 < ws(1, 1, 2) and ws(1, 1, 64) < ws(1, 8, 64) < ws(1, 8, 128) < ws(2, 8, 128)
+    # tokens, two lineage tables and two finished sets of [R][max_length] int32 dominate
+    assert ws(5, 128, 512) >= 5 * 128 * 512 * 4 * 5
+
+
+@needs_no_gpu
+def test_search_entry_rejects_bad_input_before_touching_a_device(rpx_lib):
+    """rpx_debug_search applies rpx_seq2seq_generate's checks with `vocab` in place of the decoder's vocab_size,
+    before any CUDA call; valid arguments reach the device, and there is none."""
+    buf = (C.c_uint8 * 4096)()
+    ws = C.addressof(buf) + (-C.addressof(buf)) % 256  # 256-byte aligned inside buf
+    out_len, steps = C.c_int32(0), C.c_int32(0)
+
+    def call(B=2, nb=4, V=384, n_ret=2, ML=8, eos=1, start=0, logits=ws, seqs=ws, scores=ws, nbytes=1 << 30):
+        return rpx_lib.rpx_debug_search(logits, B, nb, V, n_ret, ML, 1.0, eos, start, seqs, scores, C.byref(out_len),
+                                        C.byref(steps), None, ws, nbytes, None)
+
+    INV, UNS = _native.RPX_ERR_INVALID, _native.RPX_ERR_UNSUPPORTED
+    assert call(logits=None) == INV and call(seqs=None) == INV
+    assert call(scores=None) == INV                        # beam search needs scores
+    assert call(B=0) == INV and call(V=0) == INV
+    assert call(nb=129, n_ret=1) == INV                    # more than 128 beams
+    assert call(n_ret=5) == INV and call(n_ret=0) == INV   # num_return outside [1, num_beams]
+    assert call(nb=128, V=255, n_ret=1) == INV             # 2 nb > vocab
+    assert call(ML=1) == INV
+    assert call(eos=384) == INV and call(start=-1) == INV
+    assert call(nb=128, V=448, n_ret=1) == UNS             # nb V keys exceed one CTA's shared memory
+    assert "shared memory" in _native.last_error()
+    assert call(nbytes=64) == _native.RPX_ERR_WORKSPACE
+    for kw in ({}, {"nb": 128, "V": 416, "n_ret": 128}, {"nb": 128, "V": 256, "n_ret": 1}, {"nb": 1, "n_ret": 1, "V": 7}):
+        assert call(**kw) == _native.RPX_ERR_CUDA and _native.last_error(), kw
 
 
 def test_relative_attention_config_bound(rpx_lib):

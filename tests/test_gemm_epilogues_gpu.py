@@ -3,7 +3,9 @@ the same tile-shape dispatch as forward_layer()), on both paths and every tile s
 against the float64 reference and rounding-aware checker of tests/gemm_ref.py.
 
 Sites: QKV (RMSNorm row scale, bf16 store), O-proj and FFN-down (fp32 residual update, bf16 copy, partial
-sums of h^2 for the next RMSNorm), FFN-up (gated GELU over the interleaved gate / linear rows).  On top of
+sums of h^2 for the next RMSNorm), FFN-up (gated GELU over the interleaved gate / linear rows), and the generator's
+output head (row scale, fp32 store; on the throughput core with either layout of partial sums, as the teacher-forced
+forward and the decode steps run it).  On top of
 the per-site checks: chained launches under programmatic dependent launch, the L2-prefetch helper CTAs of
 the latency QKV projection, and bit-identical rows across tile shapes.
 
@@ -22,20 +24,22 @@ from tests import gemm_ref as R
 
 pytestmark = pytest.mark.gpu
 
-# (d_model, d_ff, heads)
+# (d_model, d_ff, heads, vocab)
 GEOMS = {
-    "byt5_small": (1472, 3584, 6),  # 64-column tail on 128-wide tiles; 46 latency parts (two RowScale batches)
-    "d768": (768, 2048, 12),  # exactly 24 latency parts
-    "byt5_base_like": (1536, 3968, 12),  # d_ff an odd multiple of 128: split-B tiles start at unit 64 of a block
-    "tiny": (64, 128, 1),  # one tile narrower than the tile width
+    "byt5_small": (1472, 3584, 6, 384),  # 64-column tail on 128-wide tiles; 46 latency parts (two RowScale batches);
+                                         # the head's last n-tile is 128 columns wide
+    "d768": (768, 2048, 12, 32128),  # exactly 24 latency parts; T5's vocabulary
+    "byt5_base_like": (1536, 3968, 12, 416),  # d_ff an odd multiple of 128: split-B tiles start at unit 64 of a
+                                              # block; the head's last n-tile is 160 columns on a 192-wide MMA
+    "tiny": (64, 128, 1, 32),  # one tile narrower than the tile width; the head is one 64-wide MMA over 32 columns
 }
 # BM = 64 / 128 switch at 384, FFN-up 32 / 64 hidden units per tile at 128, ragged tiles
 LAT_T = [1, 17, 63, 64, 65, 127, 128, 129, 383, 384, 385, 700, 1025]
 # PDL on up to 16384 tokens; 40000 gives many tiles per persistent CTA on both cores
 THR_T = [1, 129, 1000, 16384, 16385, 40000]
-SITES = ("qkv", "oproj", "ffn_up", "ffn_down")
+SITES = ("qkv", "oproj", "ffn_up", "ffn_down", "head")
 SITE_ID = {"qkv": _native.RPX_EGEMM_QKV, "oproj": _native.RPX_EGEMM_OPROJ, "ffn_up": _native.RPX_EGEMM_FFN_UP,
-           "ffn_down": _native.RPX_EGEMM_FFN_DOWN}
+           "ffn_down": _native.RPX_EGEMM_FFN_DOWN, "head": _native.RPX_EGEMM_HEAD}
 PAD = 2  # sentinel rows below every output
 EPS = float(torch.tensor(1e-6, dtype=torch.float32))
 
@@ -50,9 +54,10 @@ def _accuracy_artefact(out_dir):
 
 def _dims(site, geom):
     """(N, K, d_model) of one site."""
-    D, F, H = GEOMS[geom]
+    D, F, H, V = GEOMS[geom]
     inner = 64 * H
-    return {"qkv": (3 * inner, D, D), "oproj": (D, inner, D), "ffn_up": (2 * F, D, D), "ffn_down": (D, F, D)}[site]
+    return {"qkv": (3 * inner, D, D), "oproj": (D, inner, D), "ffn_up": (2 * F, D, D), "ffn_down": (D, F, D),
+            "head": (V, D, D)}[site]
 
 
 def _ptr(t):
@@ -84,12 +89,13 @@ class Case:
         else:
             self.B = (torch.randn(N, K, generator=g, device=dev) / math.sqrt(K)).to(torch.bfloat16)
         self.P = R.ss_parts(D, latency)
-        if site in ("qkv", "ffn_up"):
+        if site in ("qkv", "ffn_up", "head"):
             ms = torch.exp(torch.empty(T, device=dev).uniform_(math.log(1 / 4), math.log(4), generator=g))
             w = torch.rand(self.P, T, generator=g, device=dev) + 0.1
             self.ss_in = (w / w.sum(0) * ms * D).float().contiguous()
             cols = N // 2 if site == "ffn_up" else N
-            self.out = torch.full((T + PAD, cols), float("nan"), dtype=torch.bfloat16, device=dev)
+            dtype = torch.float32 if site == "head" else torch.bfloat16
+            self.out = torch.full((T + PAD, cols), float("nan"), dtype=dtype, device=dev)
         else:
             self.h32_in = torch.randn(T, N, generator=g, device=dev)
             self.h32 = torch.full((T + PAD, N), float("nan"), device=dev)
@@ -115,7 +121,7 @@ class Case:
         T = self.T
         if self.site == "ffn_up":
             return (128, 128) if not self.latency else (128, 32 if T <= 128 else 64)
-        if not self.latency:
+        if not self.latency or self.site == "head":
             return (128, 128)
         return (64 if T <= 384 else 128, 64)
 
@@ -128,6 +134,10 @@ class Case:
             ss = self.ss_in if ss_in is None else ss_in
             found = [R.check_qkv(self.out[:T], A, self.B, ss, self.D, EPS, stats),
                      R.check_sentinels("out.pad", self.out, T * self.N, R.BF16_NAN_BITS)]
+        elif self.site == "head":
+            ss = self.ss_in if ss_in is None else ss_in
+            found = [R.check_head(self.out[:T], A, self.B, ss, self.D, EPS, stats),
+                     R.check_sentinels("out.pad", self.out, T * self.N, R.F32_NAN_BITS)]
         elif self.site == "ffn_up":
             ss = self.ss_in if ss_in is None else ss_in
             found = [R.check_ffn_up(self.out[:T], A, self.W0, self.W1, ss, self.D, EPS, stats),
@@ -291,7 +301,8 @@ def test_throughput_rows_do_not_depend_on_T(rpx_lib, cuda_device, site):
         _same_rows(rpx_lib, Case(site, "byt5_small", 1000, False, 47, cuda_device), T)
 
 
-def test_entry_point_rejects_bad_input(rpx_lib, cuda_device):
+def test_entry_point_rejects_bad_site_and_input(rpx_lib, cuda_device):
+    """Sites outside [RPX_EGEMM_QKV, RPX_EGEMM_HEAD] and incomplete arguments are refused, and nothing is written."""
     t = torch.zeros(4096, dtype=torch.float32, device=cuda_device)
     p = t.data_ptr()
     st = torch.cuda.current_stream().cuda_stream
@@ -299,7 +310,7 @@ def test_entry_point_rejects_bad_input(rpx_lib, cuda_device):
     def call(site, latency=0, N=256, K=64, ss_in=p, out=p, h32=None, h16=None, ss_out=None, pf=None):
         return rpx_lib.rpx_debug_encoder_gemm(site, latency, p, p, 4, N, K, EPS, ss_in, out, h32, h16, ss_out, pf, 64, st)
 
-    assert call(4) == _native.RPX_ERR_INVALID
+    assert call(5) == _native.RPX_ERR_INVALID
     assert call(-1) == _native.RPX_ERR_INVALID
     assert call(_native.RPX_EGEMM_QKV, ss_in=None) == _native.RPX_ERR_INVALID
     assert call(_native.RPX_EGEMM_FFN_UP, out=None) == _native.RPX_ERR_INVALID
@@ -309,5 +320,11 @@ def test_entry_point_rejects_bad_input(rpx_lib, cuda_device):
     assert call(_native.RPX_EGEMM_FFN_UP, N=384) == _native.RPX_ERR_UNSUPPORTED
     assert "multiple of 256" in _native.last_error()
     assert call(_native.RPX_EGEMM_QKV, K=96) == _native.RPX_ERR_UNSUPPORTED  # d_model = K not a multiple of 64
+    for latency in (0, 1):
+        assert call(_native.RPX_EGEMM_HEAD, latency, ss_in=None) == _native.RPX_ERR_INVALID
+        assert call(_native.RPX_EGEMM_HEAD, latency, out=None) == _native.RPX_ERR_INVALID
+        assert call(_native.RPX_EGEMM_HEAD, latency, pf=p) == _native.RPX_ERR_INVALID  # the head never prefetches
+        assert call(_native.RPX_EGEMM_HEAD, latency, N=400) == _native.RPX_ERR_UNSUPPORTED
+        assert "multiple of 32" in _native.last_error()
     torch.cuda.synchronize()
     assert torch.count_nonzero(t) == 0

@@ -184,3 +184,17 @@ def test_bf16_bracket_is_exact_away_from_boundaries():
     assert R.bf16_bracket_bad(torch.tensor([1.0 + 2 ** -7], dtype=torch.bfloat16), ref[:1], tol[:1]).all()
     off = R.bf16_bracket_bad(exact[2:] + 2 ** -6, ref[2:], tol[2:])
     assert off.all()
+
+
+def test_head_checker_accepts_fp32_model_and_catches_defects():
+    """check_head: the fp32 model of the head epilogue (fl(acc * rs)) passes on both layouts of partial sums; a
+    neighbour's row scale, a dropped k-block, two swapped fragment rows and an output rounded to bf16 fail it."""
+    A, W, ms, g = _data("qkv", seed=7)
+    for latency in (False, True):
+        ss = _ss_in(ms, latency, g)
+        assert not R.check_head(_acc(A, W, None) * _rs(ss, None)[:, None], A, W, ss, D, EPS)
+        for defect in ("neighbour_row_scale", "drop_kblock", "swap_rows_r_r8"):
+            out = _acc(A, W, defect) * _rs(ss, defect)[:, None]
+            assert R.check_head(out, A, W, ss, D, EPS), (defect, latency)
+        out = (_acc(A, W, None) * _rs(ss, None)[:, None]).bfloat16().float()
+        assert R.check_head(out, A, W, ss, D, EPS), ("bf16", latency)

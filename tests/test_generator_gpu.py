@@ -263,3 +263,81 @@ def test_errors_and_bounds(cuda_device, small_gen):
     none = torch.full_like(labels, S.IGNORE)
     out = gen(input_ids=ids, attention_mask=mask, labels=none)
     assert math.isnan(float(out.loss)) and bool((out.logits == 0).all())
+
+
+# ---------------------------------------------------------------------------------------------- log-probs vs logits
+U64 = 2.0 ** -53
+
+
+def _logprob_bound(logits: torch.Tensor, labels: torch.Tensor):
+    """Float64 sum of log_softmax(logits)[label] over each row's counted positions, and the bound on its difference
+    from the engine's sum.  Per token, token_logprob_kernel computes d = fl64(x_y - mx), s = sum_j exp(fl64(x_j - mx))
+    over V terms in fp64 and d - log s, whose error is delta_k = u |d| + 1.001 rho + 2.002 u log s + u (|d| + log s +
+    1) with rho = gamma_{V-1} + 2u + V u / e (u = 2^-53; derived in tests/test_search_step_gpu.py, which runs the same
+    arithmetic); seq_logprob_kernel adds the n counted terms in token order, gamma_n sum |lp|.  The float64 reference
+    errs by at most as much again, so tol = 2 (sum delta_k + gamma_n sum |lp|)."""
+    x = logits.double()
+    V = x.shape[-1]
+    mx = x.amax(-1, keepdim=True)
+    log_s = (torch.logsumexp(x, -1, keepdim=True) - mx)[..., 0]
+    lp = torch.log_softmax(x, -1).gather(-1, labels.clamp_min(0)[..., None])[..., 0]
+    d = (x.gather(-1, labels.clamp_min(0)[..., None])[..., 0] - mx[..., 0]).abs()
+    gamma = (V - 1) * U64 / (1 - (V - 1) * U64)
+    rho = gamma + 2 * U64 + V * U64 / math.e
+    delta = U64 * d + 1.001 * rho + 2.002 * U64 * log_s + U64 * (d + log_s + 1)
+    counted = labels != S.IGNORE
+    lp = torch.where(counted, lp, torch.zeros_like(lp))
+    n = counted.sum(1)
+    g_n = n.double() * U64 / (1 - n.double() * U64)
+    tol = 2 * (torch.where(counted, delta, torch.zeros_like(delta)).sum(1) + g_n * lp.abs().sum(1))
+    return lp.sum(1), n, tol
+
+
+def _edge_labels(cfg, seed):
+    """Rows with -100 at the first, a middle and the last position, single-token rows, rows whose only counted label is
+    at out_len - 1, and longer rows with scattered -100."""
+    g = torch.Generator().manual_seed(seed)
+    V, L = cfg["vocab_size"], 40
+
+    def rnd(n):
+        return torch.randint(3, V, (n,), generator=g).tolist()
+
+    I = S.IGNORE
+    rows = [
+        [I] + rnd(18) + [I] + rnd(19) + [I],         # -100 first, middle and last
+        rnd(1),                                       # one token
+        [I] * (L - 1) + rnd(1),                       # the only counted label at out_len - 1
+        [I] * 7 + rnd(1),                             # one counted label after -100s, in a shorter row
+        rnd(L),
+        [I, I] + rnd(5) + [I] * 3 + rnd(9),
+        rnd(1) + [I] * 20,                            # one token, then -100 to the end
+    ]
+    return rows
+
+
+@pytest.mark.parametrize("head_scale", [1.0, 3000.0], ids=["plain", "logits_span_thousands"])
+def test_sequence_log_probs_against_own_logits(tmp_path, cuda_device, head_scale):
+    """sequence_log_probs is the float64 sum of log_softmax(logits)[label] over each row's counted positions of the
+    engine's own returned logits, within the derived fp64 bound (about 1e-12 relative); the counts match and the loss
+    is -sum(lp) / sum(n).  A dropped, duplicated or misaligned token's term is off by a whole log-probability."""
+    cfg = dict(synth.tiny_config(2), num_decoder_layers=2, decoder_start_token_id=0)
+    sd = synth.random_t5_seq2seq_state_dict(cfg, seed=33)
+    sd["lm_head.weight"] = sd["lm_head.weight"] * head_scale
+    gen = T5GeneratorEngine(cfg, sd, cuda_device)
+    rows = _edge_labels(cfg, 7)
+    ids, mask, labels = S.random_batch(cfg, [50, 3, 700, 17, 129, 64, 1], rows, seed=8)
+    out = gen(input_ids=ids, attention_mask=mask, labels=labels)
+    logits = out.logits.cpu()
+    lens = S.decoder_lengths(labels)
+    spread = logits[0, :int(lens[0])].amax(-1) - logits[0, :int(lens[0])].amin(-1)
+    if head_scale > 1:
+        assert float(spread.min()) > 1000, "the scaled head must give logits spanning thousands"
+    want, n, tol = _logprob_bound(logits, labels)
+    got = out.sequence_log_probs.cpu()
+    assert torch.equal(out.num_tokens.cpu().long(), n)
+    err = (got - want).abs()
+    assert bool((err <= tol).all()), (err.tolist(), tol.tolist())
+    assert bool((tol <= 1e-11 * want.abs().clamp_min(1.0)).all()), "the bound is of order 1e-12 relative"
+    assert float(out.loss) == float(-out.sequence_log_probs.sum() / out.num_tokens.sum().double())
+    assert abs(float(out.loss) - float(-want.sum() / n.sum())) <= float(tol.sum() / n.sum())
+    gen.close()
